@@ -680,31 +680,114 @@ int64_t cn_policy_last_rows(cn_policy* p) {
   return v;
 }
 
-// Internal test hook (not part of the public header): C = act(A[M,K] W[N,K]^T + bias) through the
-// wgmma 3xFP16 kernel with B-tile rows `bn` (256 or 64), fp32 device pointers in/out.
-int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, float* dC, int M, int N, int K, int act,
-                        int bn) {
-  if ((bn != 256 && bn != 64) || M <= 0 || N <= 0 || K <= 0 || N % bn || K % TC_BK)
-    return cn_set_error("cn_internal_gemm_tc: need bn in {64,256}, M, N, K > 0, N %% bn == 0 and K %% 64 == 0");
+// Internal test hooks (not part of the public header): C = act(A[M,K] W[N,K]^T + bias) through the
+// wgmma 3xFP16 kernel with B-tile rows `bn` (256 or 64), fp32 device pointers in/out.  cn_internal_gemm_tc_ex adds
+// the epilogue and operand variants the rollout uses (zero / null = off):
+//   m_ptr, m0_ptr   device-side row count and first row (rows [*m0_ptr, *m_ptr) of the M-row extent);
+//   a_col0, a_pitch A is the column view [a_col0, a_col0 + K) of an fp32 matrix [M, a_pitch] (pitch 0 = K);
+//   out_hi, out_lo  fp16 (hi, lo) split output with leading dimension ldh (pointers already at the column offset);
+//                   dC may then be null;
+//   act_lo, act_hi  the activation applies to columns [act_lo, act_hi) only (act_hi 0 = all columns).
+int cn_internal_gemm_tc_ex(const float* dA, const float* dW, const float* dbias, float* dC, int M, int N, int K, int act,
+                           int bn, const int* m_ptr, const int* m0_ptr, int a_col0, int a_pitch, __half* out_hi,
+                           __half* out_lo, int ldh, int act_lo, int act_hi) {
+  if (a_pitch == 0) a_pitch = K;
+  if ((bn != 256 && bn != 64) || M <= 0 || N <= 0 || K <= 0 || N % bn || K % TC_BK || a_col0 < 0 ||
+      a_col0 + K > a_pitch || a_col0 % 8 || a_pitch % 8 || (!dC && !out_hi) || (!out_hi != !out_lo) ||
+      (out_hi && ldh < N))
+    return cn_set_error("cn_internal_gemm_tc_ex: need bn in {64,256}, M, N, K > 0, N %% bn == 0, K %% 64 == 0, "
+                        "a_col0 + K <= a_pitch (both multiples of 8), an output and ldh >= N");
   cn_policy tmp;
   tmp.launches = 0;
   tmp.st2 = nullptr; tmp.st3 = nullptr;
   tmp.num_sms = 132; tmp.qkv_chunks = 1; tmp.launch_error = false; tmp.pdl = false;
   cudaDeviceGetAttribute(&tmp.num_sms, cudaDevAttrMultiProcessorCount, 0);
-  TcMat A, B;
-  int rc = tc_alloc(&tmp, A, M, K, TC_BM);
+  TcMat Af, A, B;
+  int rc = tc_alloc(&tmp, Af, M, a_pitch, TC_BM);
+  if (!rc) rc = tc_view(A, Af, a_col0, M, K, TC_BM);
   if (!rc) rc = tc_alloc(&tmp, B, N, K, bn);
   if (!rc) rc = tc_set_attrs();
   if (!rc) {
-    split16(&tmp, 0, dA, 1.0f, A.hi, A.lo, (size_t)M * K);
+    split16(&tmp, 0, dA, 1.0f, Af.hi, Af.lo, (size_t)M * a_pitch);
     split16(&tmp, 0, dW, 64.0f, B.hi, B.lo, (size_t)N * K);
-    gemm_tc(&tmp, 0, A, B, M, N, K, bn, dbias, act, out32(dC, N));
+    TcOut o = out32(dC, N);
+    o.oh = out_hi; o.ol = out_lo; o.ldh = ldh;
+    gemm_tc(&tmp, 0, A, B, M, N, K, bn, dbias, act, o, m_ptr, act_lo, act_hi > 0 ? act_hi : 1 << 30, m0_ptr);
     cudaError_t err = cudaDeviceSynchronize();
-    if (err != cudaSuccess) rc = cn_set_error("cn_internal_gemm_tc: %s", cudaGetErrorString(err));
+    if (err != cudaSuccess) rc = cn_set_error("cn_internal_gemm_tc_ex: %s", cudaGetErrorString(err));
     else if (tmp.launch_error) rc = 1;
   }
   for (void* q : tmp.allocs) cudaFree(q);
   return rc;
+}
+// the plain form: whole rows, A with pitch K, fp32 output [M, N], activation on every column
+int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, float* dC, int M, int N, int K, int act,
+                        int bn) {
+  return cn_internal_gemm_tc_ex(dA, dW, dbias, dC, M, N, K, act, bn, nullptr, nullptr, 0, 0, nullptr, nullptr, 0, 0, 0);
+}
+
+// Internal test hook (not part of the public header): where one named workspace buffer of the policy forward lives,
+// so a test can read every stage's input and output back after cn_policy_act.  *kind = 0: fp32 at *ptr; 1: fp16
+// (hi, lo) pair at *ptr / *ptr_lo (value = hi + lo); 2: int32.  Row r of the buffer starts at element r * *ld.
+//   row_start [N + 1], row_env [Mc], mc [1]: compacted row layout (rows of environment e: row_start[e] .. [e + 1])
+//   e1 [Mc,128], e2 [Mc,512], qkv [Mc,1536] (not in the fused kernel's mode), ao [Mc,512], sout [Mc,256]
+//   rs [N,256], t1 [N,128], u [N,256], wv [N,256], h0 [N,128], gi / gh [N,384], h1 [N,128], ac1 [N,512],
+//   a2 / c2 [N,256];  folded weights Wqkv [1536,512], bqkv, Wos [256,512], bos, Woac [512,128], boac.
+// In gemm_mode 1 a name gives what the tensor-core consumer reads (the split pair where there is one);
+// "t1.f32", "wv.f32" and "h0.f32" give the fp32 copies that are also written there.  Overwritten buffers:
+//   t1: the GRU input [enc | emb].  The edge embedding (stage gru) overwrites the te half of [enc | te]; in
+//       gemm_mode 1 only the split pair is overwritten and "t1.f32" keeps [enc | te].
+//   h1: gemm_mode 1 only (gemm_mode 0 reads the caller's h_out).
+int cn_internal_policy_buffer(cn_policy* p, const char* name, void** ptr, void** ptr_lo, int* rows, int* cols, int* ld,
+                              int* kind) {
+  if (!p || !name || !ptr || !ptr_lo || !rows || !cols || !ld || !kind)
+    return cn_set_error("cn_internal_policy_buffer: null argument");
+  const bool tcm = p->cfg.gemm_mode == 1;
+  const int N = p->N, M = p->M;
+  const std::string s(name);
+  *ptr_lo = nullptr;
+  auto f32 = [&](const float* q, int r, int c, int l) { *ptr = (void*)q; *rows = r; *cols = c; *ld = l; *kind = 0; return 0; };
+  auto i32 = [&](const int* q, int r) { *ptr = (void*)q; *rows = r; *cols = 1; *ld = 1; *kind = 2; return 0; };
+  auto f16 = [&](const TcMat& t, int r, int c) {
+    *ptr = t.hi; *ptr_lo = t.lo; *rows = r; *cols = c; *ld = t.pitch; *kind = 1; return 0;
+  };
+  if (s == "row_start") return i32(p->row_start, N + 1);
+  if (s == "row_env") return i32(p->row_env, M);
+  if (s == "mc") return i32(p->mc, 1);
+  if (s == "e1") return tcm ? f16(p->tE1, M, 128) : f32(p->e1, M, 128, 128);
+  if (s == "e2") return tcm ? f16(p->tE2, M, 512) : f32(p->e2, M, 512, 512);
+  if (s == "qkv") {
+    if (p->fuse_qkv) return cn_set_error("cn_internal_policy_buffer: 'qkv' is never written by the fused QKV-attention kernel");
+    return f32(p->qkv, M, 1536, 1536);
+  }
+  if (s == "ao") return tcm ? f16(p->tAo, M, 512) : f32(p->ao, M, 512, 512);
+  if (s == "sout") return f32(p->sout, M, 256, 256);
+  if (s == "rs") return tcm ? f16(p->tRs, N, 256) : f32(p->rs, N, 256, 256);
+  if (s == "t1") return tcm ? f16(p->tT1, N, 128) : f32(p->t1, N, 128, 128);
+  if (s == "u") return f32(p->u, N, 256, 256);
+  if (s == "wv") return tcm ? f16(p->tWv, N, 256) : f32(p->wv, N, 256, 256);
+  if (s == "h0") return tcm ? f16(p->tH0, N, 128) : f32(p->h0, N, 128, 128);
+  if (s == "gi") return f32(p->gi, N, 384, 384);
+  if (s == "gh") return f32(p->gh, N, 384, 384);
+  if (s == "h1") {
+    if (!tcm) return cn_set_error("cn_internal_policy_buffer: 'h1' exists in gemm_mode 1 only (gemm_mode 0 reads h_out)");
+    return f16(p->tH1, N, 128);
+  }
+  if (s == "ac1") return tcm ? f16(p->tAc1, N, 512) : f32(p->ac1, N, 512, 512);
+  if (s == "a2") return f32(p->a2, N, 256, 256);
+  if (s == "c2") return f32(p->c2, N, 256, 256);
+  if (tcm && s == "t1.f32") return f32(p->t1, N, 128, 128);
+  if (tcm && s == "wv.f32") return f32(p->wv, N, 256, 256);
+  if (tcm && s == "h0.f32") return f32(p->h0, N, 128, 128);
+  if (!p->finalized && (s == "Wqkv" || s == "bqkv" || s == "Wos" || s == "bos" || s == "Woac" || s == "boac"))
+    return cn_set_error("cn_internal_policy_buffer: '%s' needs cn_policy_finalize first", name);
+  if (s == "Wqkv") return f32(p->Wqkv, 1536, 512, 512);
+  if (s == "bqkv") return f32(p->bqkv, 1536, 1, 1);
+  if (s == "Wos") return f32(p->Wos, 256, 512, 512);
+  if (s == "bos") return f32(p->bos, 256, 1, 1);
+  if (s == "Woac") return f32(p->Woac, 512, 128, 128);
+  if (s == "boac") return f32(p->boac, 512, 1, 1);
+  return cn_set_error("cn_internal_policy_buffer: unknown buffer '%s' (gemm_mode %d)", name, p->cfg.gemm_mode);
 }
 
 }  // extern "C"

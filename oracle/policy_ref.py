@@ -80,16 +80,17 @@ class PolicyRef(nn.Module):
     @staticmethod
     def _len_mask(n, H):
         # create_attn_mask: first n entries valid
-        return torch.arange(H)[None, :] < n[:, None]
+        return torch.arange(H, device=n.device)[None, :] < n[:, None]
 
     def forward(self, obs, h, masks):
         b = self.base
-        sp = obs["spatial_edges"].float()
+        dt = b.robot_linear[0].weight.dtype                              # float32, or float64 after .double()
+        sp = obs["spatial_edges"].to(dt)
         N, H, _ = sp.shape
         n = obs["detected_human_num"].reshape(N).to(torch.int64)
         valid = self._len_mask(n, H)                                     # [N,H]
         robot_states = b.robot_linear(torch.cat([obs["temporal_edges"].reshape(N, 2),
-                                                 obs["robot_node"].reshape(N, 7)], -1).float())   # [N,256]
+                                                 obs["robot_node"].reshape(N, 7)], -1).to(dt))   # [N,256]
         # human-human self attention (sequence-first MultiheadAttention with key_padding_mask)
         sa = b.spatial_attn
         emb = sa.embedding_layer(sp).transpose(0, 1)                     # [H,N,512]
@@ -109,7 +110,7 @@ class PolicyRef(nn.Module):
         enc = torch.relu(r.encoder_linear(robot_states))
         edg = torch.relu(r.edge_attention_embed(weighted))
         x = torch.cat([enc, edg], -1).unsqueeze(0)                       # [1,N,128]
-        h0 = (h.reshape(N, 128) * masks.reshape(N, 1)).unsqueeze(0)
+        h0 = (h.reshape(N, 128) * masks.reshape(N, 1)).to(dt).unsqueeze(0)
         y, h1 = r.gru(x, h0)
         out = r.output_linear(y[0])                                      # [N,256]
         value = b.critic_linear(b.critic(out))
