@@ -14,7 +14,7 @@ class CnConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "num_envs", "nenv_total", "rank_offset", "seed", "human_num", "predict_steps", "const_vel",
         "randomize_attributes", "random_goal_changing", "end_goal_changing", "sort_humans", "device",
-        "phase", "val_size", "test_size", "human_num_range", "human_policy", "reserved1")] + \
+        "phase", "val_size", "test_size", "human_num_range", "human_policy", "robot_policy")] + \
         [(n, C.c_double) for n in (
             "time_step", "time_limit", "pred_timestep", "circle_radius", "arena_size",
             "discomfort_dist", "discomfort_penalty_factor", "success_reward", "collision_penalty",
@@ -78,7 +78,7 @@ def default_config_dict(**over):
     d = dict(
         num_envs=16, nenv_total=16, rank_offset=0, seed=425, human_num=20, predict_steps=5, const_vel=1,
         randomize_attributes=0, random_goal_changing=0, end_goal_changing=1, sort_humans=1, device=0,
-        phase=0, val_size=100, test_size=500, human_num_range=0, human_policy=0, reserved1=0,
+        phase=0, val_size=100, test_size=500, human_num_range=0, human_policy=0, robot_policy=0,
         time_step=0.25, time_limit=50.0, pred_timestep=0.25, circle_radius=6 * 2 ** 0.5, arena_size=6.0,
         discomfort_dist=0.25, discomfort_penalty_factor=10.0, success_reward=10.0, collision_penalty=-20.0,
         human_radius=0.3, human_v_pref=1.0, human_fov=2.0, robot_radius=0.3, robot_v_pref=1.0, robot_fov=2.0,

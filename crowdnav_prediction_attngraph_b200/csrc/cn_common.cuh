@@ -52,6 +52,7 @@ struct CnParams {
   int social_force;       // humans.policy == 'social_force' (crowd_nav/policy/social_force.py) instead of ORCA
   double sf_A, sf_B, sf_KI;   // config.sf
   int defer_tries;        // warp-scope rejection-sampling budget (cn_env_event_kernel -> cn_env_event_heavy_kernel)
+  int robot_policy;       // robot.policy: 0 caller's action, 1 'orca', 2 'social_force' (cn_robot_act)
 };
 
 // Struct-of-arrays environment state in HBM.  Per-human arrays are [N][H] (human index
@@ -60,6 +61,13 @@ struct CnState {
   // robot
   double *rpx, *rpy, *rgx, *rgy;     // fp64 like the reference's Python floats
   float *rvx, *rvy;                  // fp32-valued (clipped action)
+  double *rwx, *rwy;                 // fp64 velocity of a social-force robot (the reference keeps Python floats; rvx / rvy
+                                     // hold it narrowed, as the observation's temporal_edges read it)
+  // the robot's own rvo2 simulator (robot_policy 1): created at the environment's FIRST robot solve and never rebuilt
+  // (crowd_sim.py:184 creates robot.policy once per env process), so these survive episode installs
+  uint8_t *rsim_exists;              // [N]
+  float *rsim_nd;                    // [N] neighborDist frozen at creation (config.orca.neighbor_dist then)
+  float *rsim_rother;                // [N][H] radii of the belief rows frozen at creation (+ 0.01 + safety_space)
   double *potential;                 // -|goal - pos| bookkeeping (crowd_sim_var_num.py:351-352)
   double *fut_pen;                   // future-intrusion penalty of the STORED prediction (crowd_sim_pred.py:222-231)
   double *nd_global;                 // process-global config.orca.neighbor_dist (agent.py:21-22)

@@ -70,7 +70,9 @@ struct CnEnvSh {
   // robot + scalars
   double rpx, rpy, rgx, rgy;
   float rvx, rvy;
-  float ax, ay;          // clipped action
+  double rwx, rwy;       // social-force robot: fp64 velocity (state) and the one computed for this step
+  double nrwx, nrwy;
+  float ax, ay;          // clipped action (or the robot policy's velocity)
   double reward;
   int done, info, reset_flag;
   int nvis;
@@ -101,8 +103,89 @@ CN_HD bool cn_in_fov(double x1, double y1, double vx1, double vy1, double x2, do
 }
 
 // ------------------------------------------------------------------------------------------
+// Robot policy inside the step (robot_policy != 0; crowd_sim_var_num.py:371-377: the env ignores the incoming action and
+// calls robot.act(last_human_states)).  Leader thread, serial, at the end of cn_phase_load of a step, on the state the
+// previous step left behind: the robot's position / velocity just loaded into s and its belief rows bpx..brad in HBM,
+// which the step rewrites only in cn_phase_obs_a, after the reward.  Sets s.ax / s.ay (fp32 velocity) and, for social
+// force, s.nrwx / s.nrwy (fp64), which cn_phase_reward integrates.
+//
+// 'orca' (crowd_nav/policy/orca.py:64-117, the robot as agent 0 of its own rvo2 simulator): neighbours are ALL H belief
+// rows narrowed to float, including the (15, 15, 0, 0, 0.3) rows and the dead-reckoned rows of unseen humans (no FOV
+// test, no (7, 7) dummy); maxNeighbors = H; own radius robot.radius + 0.01 + safety_space, maxSpeed robot.v_pref; the
+// other radii and neighborDist are frozen when the simulator is created (rsim_*); the result is applied unclipped.
+// 'social_force' (crowd_nav/policy/social_force.py): pull towards the goal with v_pref, push from every belief row, fp64
+// in the reference's expression order, speed clipped to v_pref.
+template <int MAXH>
+CN_HD_NOINLINE void cn_robot_act(const CnParams& p, const CnState& g, CnEnvSh& s, int e) {
+  const int H = p.H;
+  const size_t row = (size_t)e * H;
+  if (p.robot_policy == 2) {
+    const double px = s.rpx, py = s.rpy, vx = s.rwx, vy = s.rwy, vp = p.robot_vpref;
+    const double dx = s.rgx - px, dy = s.rgy - py;
+    const double dist = sqrt(dx * dx + dy * dy);
+    const double dvx = p.sf_KI * ((dx / dist) * vp - vx);
+    const double dvy = p.sf_KI * ((dy / dist) * vp - vy);
+    double ivx = 0.0, ivy = 0.0;
+    for (int j = 0; j < H; ++j) {
+      const double ex = px - g.bpx[row + j], ey = py - g.bpy[row + j];
+      const double d = sqrt(ex * ex + ey * ey);
+      const double w = p.sf_A * exp((p.robot_radius + g.brad[row + j] - d) / p.sf_B);
+      ivx += w * (ex / d);
+      ivy += w * (ey / d);
+    }
+    double nvx = vx + (dvx + ivx) * p.time_step;
+    double nvy = vy + (dvy + ivy) * p.time_step;
+    const double nrm = cn_norm_dot(nvx, nvy);                  // np.linalg.norm([new_vx, new_vy])
+    if (nrm > vp) { nvx = nvx / nrm * vp; nvy = nvy / nrm * vp; }
+    s.nrwx = nvx; s.nrwy = nvy;
+    s.ax = (float)nvx; s.ay = (float)nvy;
+    return;
+  }
+  const double pad = 0.01;
+  if (!g.rsim_exists[e]) {                                     // first solve of this environment: create the simulator
+    g.rsim_nd[e] = (float)g.nd_global[e];
+    for (int j = 0; j < H; ++j) g.rsim_rother[row + j] = (float)(g.brad[row + j] + pad + p.orca_safety_space);
+    g.rsim_exists[e] = 1;
+  }
+  const float nd = g.rsim_nd[e];
+  const float rself = (float)(p.robot_radius + pad + p.orca_safety_space);
+  const float vmax = (float)p.robot_vpref;
+  const double dvx = s.rgx - s.rpx, dvy = s.rgy - s.rpy;
+  const double speed = cn_norm_dot(dvx, dvy);
+  const CnF2 pref = speed > 1 ? f2((float)(dvx / speed), (float)(dvy / speed)) : f2((float)dvx, (float)dvy);
+  const CnF2 pos = f2((float)s.rpx, (float)s.rpy);
+  const CnF2 vel = f2(s.rvx, s.rvy);
+  const float rangeSq = nd * nd;
+  const float invTimeHorizon = 1.0f / p.orca_time_horizon;
+  const float timeStep = (float)p.time_step;
+  // neighbours inside neighborDist, ascending distance, ties in index order; counting rank as in cn_orca_build
+  float vd[MAXH];
+  uint8_t vj[MAXH];
+  int nl = 0;
+  for (int j = 0; j < H; ++j) {
+    const float d = f2abssq(f2sub(pos, f2((float)g.bpx[row + j], (float)g.bpy[row + j])));
+    if (d < rangeSq) { vd[nl] = d; vj[nl] = (uint8_t)j; ++nl; }
+  }
+  CnLocalLines<MAXH> lines;
+  for (int a = 0; a < nl; ++a) {
+    const float da = vd[a];
+    int rank = 0;
+    for (int b = 0; b < nl; ++b) rank += (vd[b] < da || (vd[b] == da && b < a)) ? 1 : 0;
+    const size_t i = row + vj[a];
+    lines.set(rank, cn_orca_line(pos, vel, rself, f2((float)g.bpx[i], (float)g.bpy[i]), f2((float)g.bvx[i], (float)g.bvy[i]),
+                                 g.rsim_rother[i], invTimeHorizon, timeStep));
+  }
+  CnF2 result;
+  const int fail = cn_lp2(lines, nl, vmax, pref, false, result);
+  if (fail < nl) cn_lp3<MAXH>(lines, nl, fail, vmax, result);
+  s.ax = result.x; s.ay = result.y;
+}
+
+// ------------------------------------------------------------------------------------------
 // Phase LOAD: every (env, human) thread loads its human; the leader (h == 0) loads the robot
-// and clips the action (srnn.py:17-33, fp32).
+// and clips the action (srnn.py:17-33, fp32), or with robot_policy != 0 runs the robot's own policy instead.
+// ROBOT = false (the step kernel of a network policy) compiles the robot policy out; MAXH bounds its neighbour arrays.
+template <int MAXH = 128, bool ROBOT = true>
 CN_HD void cn_phase_load(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h,
                          const float* action /* [N,2] or null (reset) */) {
   const size_t i = cn_idx(p, e, h);
@@ -114,9 +197,12 @@ CN_HD void cn_phase_load(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
   if (h == 0) {
     s.rpx = g.rpx[e]; s.rpy = g.rpy[e]; s.rgx = g.rgx[e]; s.rgy = g.rgy[e];
     s.rvx = g.rvx[e]; s.rvy = g.rvy[e];
+    if (p.robot_policy == 2) { s.rwx = g.rwx[e]; s.rwy = g.rwy[e]; }
     s.done = 0; s.info = 0; s.reward = 0.0; s.reset_flag = 0; s.nvis = 0; s.goal_flag = 0; s.lp3_cost = 0;
     s.hn = g.hn[e];
-    if (action) {
+    if (ROBOT && action && p.robot_policy) {
+      cn_robot_act<MAXH>(p, g, s, e);
+    } else if (action) {
       float ax = action[2 * e], ay = action[2 * e + 1];
       const float nrm = sqrtf(ax * ax + ay * ay);          // np.linalg.norm(float32[2])
       const float vp = (float)p.robot_vpref;
@@ -338,8 +424,14 @@ CN_HD void cn_phase_reward(const CnParams& p, const CnState& g, CnEnvSh& s, int 
   if (out.not_done) out.not_done[e] = done ? 0.0f : 1.0f;
   if (done) { out.ep_ret[e] = ret; out.ep_len[e] = len; }
   // robot.step(action) (agent.py:170-183); time
-  s.rpx = s.rpx + (double)s.ax * p.time_step;
-  s.rpy = s.rpy + (double)s.ay * p.time_step;
+  if (p.robot_policy == 2) {
+    s.rpx = s.rpx + s.nrwx * p.time_step;
+    s.rpy = s.rpy + s.nrwy * p.time_step;
+    s.rwx = s.nrwx; s.rwy = s.nrwy;
+  } else {
+    s.rpx = s.rpx + (double)s.ax * p.time_step;
+    s.rpy = s.rpy + (double)s.ay * p.time_step;
+  }
   s.rvx = s.ax; s.rvy = s.ay;
   g.step_count[e] = step + 1;
 }
@@ -680,7 +772,8 @@ CN_HD void cn_install_env(const CnParams& p, const CnState& g, CnEnvSh& s, int e
   for (int w = h; w < 624; w += H) g.mt[(size_t)e * 624 + w] = g.prep_mt[(size_t)e * 624 + w];
   if (h == 0) {
     const double* r = g.prep_robot + (size_t)e * 4;
-    s.rpx = r[0]; s.rpy = r[1]; s.rgx = r[2]; s.rgy = r[3]; s.rvx = 0.0f; s.rvy = 0.0f;
+    s.rpx = r[0]; s.rpy = r[1]; s.rgx = r[2]; s.rgy = r[3]; s.rvx = 0.0f; s.rvy = 0.0f; s.rwx = 0.0; s.rwy = 0.0;
+    // the robot's rvo2 simulator (rsim_*) is NOT reset: robot.policy outlives the episode
     // case_counter = (case_counter + nenv) % case_size[phase]  (train: UINT32_MAX - 2000, test: env.test_size)
     g.case_counter[e] = (uint32_t)(((uint64_t)g.case_counter[e] + (uint64_t)p.nenv_total) % (uint64_t)p.case_size);
     g.potential[e] = -fabs(cn_norm_dot(s.rgx - s.rpx, s.rgy - s.rpy));
@@ -755,7 +848,8 @@ CN_HD void cn_phase_obs_a(const CnParams& p, const CnState& g, CnEnvSh& s, int e
     return;
   }
   const double dist = cn_norm_dot(s.rpx - s.px[h], s.rpy - s.py[h]) - p.robot_radius - s.rad[h];
-  const bool in_fov = cn_in_fov(s.rpx, s.rpy, s.rvx, s.rvy, s.px[h], s.py[h], p.robot_fov);
+  const double rvx = p.robot_policy == 2 ? s.rwx : (double)s.rvx, rvy = p.robot_policy == 2 ? s.rwy : (double)s.rvy;
+  const bool in_fov = cn_in_fov(s.rpx, s.rpy, rvx, rvy, s.px[h], s.py[h], p.robot_fov);
   const bool vis = in_fov && (dist <= p.sensor_range);
   s.visr[h] = vis ? 1 : 0;
   g.vis[i] = vis ? 1 : 0;
@@ -895,5 +989,6 @@ CN_HD void cn_phase_store(const CnParams& p, const CnState& g, const CnEnvSh& s,
   if (h == 0) {
     g.rpx[e] = s.rpx; g.rpy[e] = s.rpy; g.rgx[e] = s.rgx; g.rgy[e] = s.rgy;
     g.rvx[e] = s.rvx; g.rvy[e] = s.rvy;
+    if (p.robot_policy == 2) { g.rwx[e] = s.rwx; g.rwy[e] = s.rwy; }
   }
 }

@@ -67,7 +67,9 @@ __device__ inline CnEnvSh* env_view(unsigned char* base, const EnvSmemLayout& L,
 // One rollout step of every environment.  Episodes that finish INSTALL their prepared successor
 // (g.prep_*, computed off the critical path by cn_env_event_kernel) and emit its first observation in
 // the same launch.  mode 1 = reset of the whole vector env: no step, every environment installs.
-template <int MAXH, int MAXW>
+// ROBOT: robot_policy != 0 (the robot's ORCA / social-force solve, cn_robot_act); a separate instantiation so the network
+// policy's kernel carries none of its code.
+template <int MAXH, int MAXW, bool ROBOT>
 __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState g, const float* __restrict__ action,
                                                           CnObs ob, CnStepOut out, int epb, int line_cap, int mode) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -115,7 +117,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
   if (mode == 1) {
     if (active && h == 0) { s->done = 1; s->info = 0; s->reward = 0.0; s->reset_flag = 0; s->nvis = 0; s->goal_flag = 0; s->lp3_cost = 0; s->hn = 0; }
   } else if (active) {
-    cn_phase_load(p, g, *s, e, h, mode == 3 ? nullptr : action);
+    cn_phase_load<MAXH, ROBOT>(p, g, *s, e, h, mode == 3 ? nullptr : action);   // ROBOT: + the robot's own policy
   }
   __syncthreads();
   // live = this thread's slot holds a human (slots [hn, H) are empty when sim.human_num_range > 0)
@@ -462,10 +464,15 @@ int dev_alloc(cn_env* env, const char* name, T** ptr, size_t count) {
 
 typedef void (*KernelFn)(CnParams, CnState, const float*, CnObs, CnStepOut, int, int, int);
 
-KernelFn pick_kernel(int maxh) {
-  if (maxh <= 32) return cn_env_step_kernel<32, 16>;
-  if (maxh <= 64) return cn_env_step_kernel<64, 16>;
-  return cn_env_step_kernel<128, 16>;
+KernelFn pick_kernel(int maxh, bool robot) {
+  if (robot) {
+    if (maxh <= 32) return cn_env_step_kernel<32, 16, true>;
+    if (maxh <= 64) return cn_env_step_kernel<64, 16, true>;
+    return cn_env_step_kernel<128, 16, true>;
+  }
+  if (maxh <= 32) return cn_env_step_kernel<32, 16, false>;
+  if (maxh <= 64) return cn_env_step_kernel<64, 16, false>;
+  return cn_env_step_kernel<128, 16, false>;
 }
 
 CnObs to_obs(const cn_obs_ptrs* o) {
@@ -518,7 +525,7 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
     env->prep_dirty = false;
   }
   const int grid = (env->p.N + env->epb - 1) / env->epb;
-  KernelFn fn = pick_kernel(env->maxh);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0);
   // mode 0 with a pre-solve of this state done on the side stream (joined above) -> finishing pass only (mode 2)
   const int kmode = (mode == 0 && env->presolved) ? 2 : mode;
   env->presolved = false;
@@ -640,6 +647,16 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
     return cn_set_error("cn_env_create: social-force humans are covered in phase 'train' only (the test phase's "
                         "ground-truth look-ahead runs the ORCA solver)");
   }
+  if (cfg->robot_policy < 0 || cfg->robot_policy > 2) {
+    cn_env_destroy(env);
+    return cn_set_error("cn_env_create: robot_policy %d unsupported (0 = the caller's action, 1 = 'orca', 2 = 'social_force')",
+                        cfg->robot_policy);
+  }
+  if (cfg->robot_policy != 0 && (cfg->const_vel || cfg->human_num_range > 0)) {
+    cn_env_destroy(env);
+    return cn_set_error("cn_env_create: the ORCA / social-force robot is covered for CrowdSimVarNum-v0 (const_vel 0) with "
+                        "human_num_range 0");
+  }
   if (cfg->phase != 0 && cfg->phase != 2) {
     cn_env_destroy(env);
     return cn_set_error("cn_env_create: phase %d unsupported (0 = 'train', 2 = 'test')", cfg->phase);
@@ -656,6 +673,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   p.orca_time_horizon = (float)cfg->orca_time_horizon;
   p.social_force = cfg->human_policy == 1 ? 1 : 0;
   p.sf_A = cfg->sf_A; p.sf_B = cfg->sf_B; p.sf_KI = cfg->sf_KI;
+  p.robot_policy = cfg->robot_policy;
   {
     // warp-scope budget of rejection-sampling tries before an event goes to the CTA-scope kernel
     // (CN_DEFER_TRIES=1 sends every search that needs a second candidate there: parity tests of the heavy path)
@@ -682,6 +700,8 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   A(lp_cost, N); A(defer_list, N); A(defer_ctl, 8); A(hn, N); A(prep_hn, N); A(sim_n, NH);
   A(pre_vx, NH); A(pre_vy, NH); A(pre_nlf, NH);
   A(hwx, cfg->human_policy ? NH : (size_t)4); A(hwy, cfg->human_policy ? NH : (size_t)4);
+  A(rwx, cfg->robot_policy == 2 ? N : (size_t)4); A(rwy, cfg->robot_policy == 2 ? N : (size_t)4);
+  A(rsim_exists, N); A(rsim_nd, N); A(rsim_rother, cfg->robot_policy == 1 ? NH : (size_t)4);
 #undef A
   if (!rc) {
     // nd_global starts at the configured value (config.orca.neighbor_dist)
@@ -721,7 +741,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   const EnvSmemLayout L = env_layout(p.H, true, p.social_force != 0);
   int nsm = 0;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-  KernelFn fn = pick_kernel(env->maxh);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0);
   err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(err)); }
   const int cap_max = p.H > 1 ? p.H - 1 : 1;

@@ -51,6 +51,16 @@ def _summary(test_size, time_limit, end_codes, end_times, path_len, too_close_ra
     return out
 
 
+def _act(actor_critic, obs, hxs, masks, n, dev):
+    """(action, hxs): the policy's deterministic action and new recurrent state, or zeros for actor_critic=None (the
+    ORCA / social-force robot baselines drive the robot inside env.step; the loop passes zeros, rl/evaluation.py:64-73)."""
+    if actor_critic is None:
+        return torch.zeros(n, 2, device=dev), hxs
+    with torch.no_grad():
+        _, action, _, hxs = actor_critic.act(obs, hxs, masks, deterministic=True)
+    return action, hxs
+
+
 def evaluate(actor_critic, eval_envs, num_processes, device, test_size, logging, config, args, visualize=False):
     """rl/evaluation.py:7-160 against a CudaCrowdVecEnv with ONE environment (phase 'test').  Returns the
     metrics as a dict (the reference only logs them)."""
@@ -70,8 +80,7 @@ def evaluate(actor_critic, eval_envs, num_processes, device, test_size, logging,
         infos = None
         while not done:
             step_counter += 1
-            with torch.no_grad():
-                _, action, _, hxs = actor_critic.act(obs, hxs, masks, deterministic=True)
+            action, hxs = _act(actor_critic, obs, hxs, masks, 1, dev)
             global_time = (step_counter - 1) * dt            # baseEnv.global_time read before the step
             obs, rew, done_arr, infos = eval_envs.step(action)
             done = bool(done_arr[0])
@@ -101,14 +110,41 @@ def evaluate(actor_critic, eval_envs, num_processes, device, test_size, logging,
             raise ValueError('Invalid end signal from environment')
     out = _summary(test_size, time_limit, end_codes, end_times, all_path_len, too_close_ratios, min_dist, ep_rewards, logging)
     out["episode_steps"] = steps
+    out.update(case_code=[int(c) for c in end_codes], case_nav_time=list(end_times), case_path_len=list(all_path_len))
     return out
+
+
+def _freeze_robot_sim(base, d, dev):
+    """Create the robot's rvo2 simulator the way the sequential protocol does (first step of case 0 on a single
+    environment) and install it in every environment of `base`."""
+    one = dict(d)
+    one.update(num_envs=1)
+    env1 = CudaCrowdVecEnv(device=dev, cfg=one)
+    try:
+        env1.set_state("seed_off", np.zeros(1, np.int32))
+        env1.set_state("case_counter", np.zeros(1, np.uint32))
+        env1.reset()
+        env1.step(torch.zeros(1, 2, device=dev))
+        N, H = base.num_envs, base.human_num
+        base.set_state("rsim_exists", np.ones(N, np.uint8))
+        base.set_state("rsim_nd", np.repeat(env1.get_state("rsim_nd"), N))
+        base.set_state("rsim_rother", np.tile(env1.get_state("rsim_rother"), N))
+    finally:
+        env1.close()
 
 
 def evaluate_batched(actor_critic, config, env_name, seed, test_size, device, logging=None, cfg_dict=None, gst_params=None):
     """The same test cases as `evaluate`, as test_size parallel environments on one GPU.
     config: reference Config object (or pass cfg_dict = a flat cn_config dict).  gst_params: predictor parameters
     for CrowdSimPredRealGST-v0 + VecPretextNormalize (config 3); the wrapper's buffers start empty for every test
-    case exactly like the sequential protocol's explicit reset()."""
+    case exactly like the sequential protocol's explicit reset().
+
+    actor_critic=None runs the ORCA / social-force robot baselines (robot.policy 'orca' / 'social_force').  The
+    reference creates the robot's rvo2 simulator once per process, at the first step of case 0, and reuses it for
+    every later case; its neighborDist and radii are frozen then.  To give every parallel case those same frozen
+    parameters, one step of case 0 runs first on a one-environment handle and its robot simulator (rsim_*) is
+    uploaded to all N environments before the batch starts.  Without randomised attributes the frozen values are the
+    configured constants and the hand-off changes nothing."""
     dev = torch.device(device)
     N = test_size
     if cfg_dict is None:
@@ -121,6 +157,8 @@ def evaluate_batched(actor_critic, config, env_name, seed, test_size, device, lo
     size = int(d["test_size"])
     base.set_state("seed_off", np.zeros(N, np.int32))
     base.set_state("case_counter", ((2 * np.arange(N)) % size).astype(np.uint32))
+    if int(d.get("robot_policy", 0)) == 1:
+        _freeze_robot_sim(base, d, dev)
     time_limit, dt = float(d["time_limit"]), float(d["time_step"])
     hxs = {'human_node_rnn': torch.zeros(N, 1, 128, device=dev)}
     masks = torch.zeros(N, 1, device=dev)
@@ -138,8 +176,7 @@ def evaluate_batched(actor_critic, config, env_name, seed, test_size, device, lo
     for _ in range(max_steps):
         if not alive.any():
             break
-        with torch.no_grad():
-            _, action, _, hxs = actor_critic.act(obs, hxs, masks, deterministic=True)
+        action, hxs = _act(actor_critic, obs, hxs, masks, N, dev)
         obs, rew, done, infos = env.step(action)
         codes, aux = infos._codes, infos._aux
         pos = obs['robot_node'][:, 0, :2].cpu().numpy()
@@ -163,5 +200,10 @@ def evaluate_batched(actor_critic, config, env_name, seed, test_size, device, lo
     out = _summary(N, time_limit, end_codes, list(end_times), list(path_len), list(too_close / steps * 100), flat_min,
                    list(ep_rewards), logging)
     out["episode_steps"] = [int(x) for x in steps]
+    # per-case records (the reference logs only the aggregates): outcome, nav time, path length, too-close frames and
+    # the min distances of those frames
+    out.update(case_code=[int(c) for c in end_codes], case_nav_time=[float(x) for x in end_times],
+               case_path_len=[float(x) for x in path_len], case_too_close=[int(x) for x in too_close],
+               case_min_dist=min_dist)
     env.close()
     return out

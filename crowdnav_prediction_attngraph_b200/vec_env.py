@@ -81,6 +81,10 @@ class Box(_Space):
     pass
 
 
+# robot.policy -> cn_config.robot_policy (0: the caller's action)
+ROBOT_POLICIES = {"orca": 1, "social_force": 2}
+
+
 def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None, rank_offset=0, device_index=0,
                                phase=None, allow_unsorted=False):
     """Snapshot a reference `Config` object (crowd_nav/configs/config.py) into the flat cn_config.
@@ -101,6 +105,18 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         const_vel = 0
     else:
         raise NotImplementedError("env id %r is not covered by the CUDA engine" % env_name)
+    # robot.policy 'orca' / 'social_force': the robot is driven inside env.step and the caller's action is ignored
+    # (crowd_sim_var_num.py:371-377); any other name (a network policy) takes the caller's action
+    robot_policy = ROBOT_POLICIES.get(getattr(config.robot, "policy", None), 0)
+    if robot_policy:
+        if const_vel:
+            raise NotImplementedError(
+                "robot.policy %r on CrowdSimPred-v0 is not covered: its ORCA branch (crowd_sim_pred.py:105-116) feeds the "
+                "robot the ground-truth future trajectories ((predict_steps + 1) * human_num agents) and its "
+                "social-force branch calls clip_action on a policy that has none" % (config.robot.policy,))
+        if int(config.sim.human_num_range) > 0:
+            raise NotImplementedError("robot.policy %r with sim.human_num_range > 0 is not covered (the robot's rvo2 "
+                                      "simulator would be rebuilt as humans join and leave)" % (config.robot.policy,))
     sort_humans = getattr(getattr(config, "args", None), "sort_humans", True)
     if not sort_humans and not allow_unsorted:
         # the policy mirror masks attention with detected_human_num, which is only valid for distance-sorted rows
@@ -124,7 +140,7 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         sensor_range=float(config.robot.sensor_range), goal_change_chance=float(config.humans.goal_change_chance),
         orca_neighbor_dist=float(config.orca.neighbor_dist), orca_safety_space=float(config.orca.safety_space),
         orca_time_horizon=float(config.orca.time_horizon),
-        human_policy=1 if config.humans.policy == "social_force" else 0,
+        human_policy=1 if config.humans.policy == "social_force" else 0, robot_policy=robot_policy,
         sf_A=float(config.sf.A), sf_B=float(config.sf.B), sf_KI=float(config.sf.KI),
         phase=2 if phase == "test" else 0, val_size=int(getattr(config.env, "val_size", 100)),
         test_size=int(getattr(config.env, "test_size", 500)))
@@ -379,7 +395,8 @@ class CudaCrowdVecEnv(object):
                bpx="f8", bpy="f8", bvx="f8", bvy="f8", brad="f8", vis="u1", sim_exists="u1",
                sim_nd="f4", sim_rself="f4", sim_vmax="f4", sim_rother="f4", mt="u4", mt_pos="i4",
                last_hvx="f4", last_hvy="f4", orca_nlines="i4", orca_fail="i4", evt="u1", spawn_overflow="u1",
-               defer_ctl="i4", defer_list="i4", lp_cost="i4", hn="i4", prep_hn="i4", hwx="f8", hwy="f8")
+               defer_ctl="i4", defer_list="i4", lp_cost="i4", hn="i4", prep_hn="i4", hwx="f8", hwy="f8",
+               rwx="f8", rwy="f8", rsim_exists="u1", rsim_nd="f4", rsim_rother="f4")
 
     def get_state(self, name):
         nbytes = self.lib.cn_env_state_bytes(self._h, name.encode())
@@ -438,6 +455,9 @@ class CudaPretextVecEnv(object):
             d.update(const_vel=0, sort_humans=0)
         else:
             over.update(const_vel=0, sort_humans=0)
+        if (d if d is not None else over).get("robot_policy", 0):
+            raise NotImplementedError("the ORCA / social-force robot is not covered behind the GST wrapper "
+                                      "(VecPretextNormalize): the reference's baselines run without it")
         self.env = CudaCrowdVecEnv(num_envs=num_envs, device=device, cfg=d, **over)
         e = self.env
         self.lib, self.device, self.cfgd = e.lib, e.device, e.cfgd

@@ -60,7 +60,9 @@ typedef struct cn_config {
   int32_t human_num_range;        /* sim.human_num_range: humans join / leave every 5 s; observations are padded to
                                    * human_num + human_num_range rows (crowd_sim_pred.py:165-194)             */
   int32_t human_policy;           /* humans.policy: 0 'orca', 1 'social_force' (crowd_nav/policy/social_force.py) */
-  int32_t reserved1;
+  int32_t robot_policy;           /* robot.policy: 0 the caller's action (a network policy), 1 'orca', 2 'social_force':
+                                   * the step computes the robot's velocity itself and ignores d_action
+                                   * (crowd_sim_var_num.py:371-377); CrowdSimVarNum-v0 with human_num_range 0 only */
   double time_step, time_limit, pred_timestep;
   double circle_radius, arena_size;
   double discomfort_dist, discomfort_penalty_factor, success_reward, collision_penalty;

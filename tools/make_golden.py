@@ -57,6 +57,21 @@ CASES = {
                            randomize=True, goal_changing=True, nenv=2, steps=160, seed=21),
     "env_pred_h10_test_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="const_vel",
                                    randomize=True, goal_changing=True, nenv=2, steps=200, seed=11, phase="test"),
+    # robot.policy = 'orca' / 'social_force' (the paper's baselines, trained_models/ORCA_no_rand and SF_no_rand): the
+    # robot is driven inside env.step, the scripted action is passed and ignored; robot_vel records its velocity after
+    # every step.  The randomised train-phase cases cross episode ends, which keep the robot's frozen rvo2 simulator.
+    "env_varnum_h20_test_orca_robot": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                           robot_policy="orca", randomize=False, goal_changing=False, nenv=2, steps=120,
+                                           seed=425, phase="test"),
+    "env_varnum_h10_orca_robot_rand": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
+                                           robot_policy="orca", randomize=True, goal_changing=True, nenv=2, steps=200,
+                                           seed=31),
+    "env_varnum_h20_test_sf_robot": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                         robot_policy="social_force", randomize=False, goal_changing=False, nenv=2,
+                                         steps=120, seed=425, phase="test"),
+    "env_varnum_h10_sf_robot_rand": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
+                                         robot_policy="social_force", randomize=True, goal_changing=True, nenv=2,
+                                         steps=200, seed=31),
 }
 
 
@@ -84,6 +99,7 @@ def build_reference_env(case, rank):
     cfg.sim.human_num = case["human_num"]
     cfg.sim.human_num_range = case.get("human_num_range", 0)
     cfg.humans.policy = case.get("human_policy", "orca")
+    cfg.robot.policy = case.get("robot_policy", "selfAttn_merge_srnn")
     cfg.sim.predict_method = case["predict_method"]
     cfg.env.use_wrapper = False
     cfg.env.randomize_attributes = case["randomize"]
@@ -151,7 +167,8 @@ def run_case(name, case):
     rec = dict(actions=np.zeros((T, N, 2), np.float32), reward=np.zeros((T, N)), done=np.zeros((T, N), bool),
                info=np.zeros((T, N), np.int32), min_danger=np.zeros((T, N)),
                human_actions=np.zeros((T, N, H, 2), np.float32),
-               orca_nlines=np.zeros((T, N, H), np.int32), orca_fail=np.zeros((T, N, H), np.int32))
+               orca_nlines=np.zeros((T, N, H), np.int32), orca_fail=np.zeros((T, N, H), np.int32),
+               robot_vel=np.zeros((T, N, 2)))
     obs_keys = ["robot_node", "temporal_edges", "spatial_edges", "detected_human_num"] + \
                (["visible_masks"] if W == 2 else [])
     state_keys = ["robot", "hpx", "hpy", "hvx", "hvy", "hgx", "hgy", "hrad", "hvpref", "belief", "traj",
@@ -177,6 +194,7 @@ def run_case(name, case):
             rec["done"][t, k] = done
             rec["info"][t, k] = INFO_CODE[type(info["info"]).__name__]
             rec["min_danger"][t, k] = getattr(info["info"], "min_dist", 0.0)
+            rec["robot_vel"][t, k] = env.robot.vx, env.robot.vy
             # velocities/diagnostics of the step just taken (before a possible respawn zeroes them
             # we read the sims, which always hold the solved velocity of agent 0)
             rec["human_actions"][t, k, len(env.humans):] = np.nan
