@@ -12,10 +12,12 @@
 //
 // Tiling: one 128 x BN output tile per CTA (BN = 256 for the large per-human GEMMs, BN = 64 for the
 // per-environment layers where M is only a few thousand rows and more CTAs matter more than tile
-// efficiency), K in blocks of 64 fp16 (= one 128-byte swizzle atom), TMA->smem ring of 2 (BN=256,
-// 96 KB per stage) or 4 (BN=64, 48 KB per stage) stages.  Warp groups: 0 = TMA producer (one thread),
-// 1 and 2 = consumers: each issues wgmma.m64nBNk16 for 64 rows of the tile, keeps that 64 x BN fp32
-// accumulator in registers and runs the epilogue (bias, activation, stores) straight from them.
+// efficiency), TMA->smem ring of 4 stages of 48 KB.  BN = 64: k-blocks of 64 fp16 (one 128-byte swizzle
+// atom).  BN = 256: k-blocks of 32 fp16 (64-byte swizzle), so a slot is refilled after a quarter of the ring's
+// MMA time instead of half of it; each output element still sees the same wgmma instructions in the same order.
+// Warp groups: 0 = TMA producer (one thread), 1 and 2 = consumers: each issues wgmma.m64nBNk16 for 64 rows of the
+// tile, keeps that 64 x BN fp32 accumulator in registers and runs the epilogue (bias, activation, stores) straight
+// from them.
 //
 // PROMOTE (the PPO update's GEMMs, which must be fp32-equivalent): the tensor core sums each 64-wide k-block on its own
 // and the CUDA cores add the block sums into a second register accumulator with IEEE round-to-nearest.  wgmma's fp32
@@ -28,16 +30,18 @@
 #include <stdint.h>
 
 #define TC_BM 128
-#define TC_BK 64
-#define TC_A_TILE_BYTES (TC_BM * TC_BK * 2)           // 16 KB
+#define TC_BK 64                                      // k-block of the BN = 64 instances (and the PPO update's maps)
 #define TC_CONSUMER_WARPS 8                           // two consumer warp groups
 #define TC_THREADS (128 + 32 * TC_CONSUMER_WARPS)
 
 template <int BN>
 struct TcCfg {
-  static constexpr int kStages = (BN >= 256) ? 2 : 4;
-  static constexpr int kBTile = BN * TC_BK * 2;
-  static constexpr int kStageBytes = 2 * TC_A_TILE_BYTES + 2 * kBTile;
+  static constexpr int kBK = (BN >= 256) ? 32 : TC_BK;        // k-block width (fp16) = TMA box width
+  static constexpr int kSwizzle = 2 * kBK;                    // bytes per smem row: 64- or 128-byte swizzle
+  static constexpr int kStages = 4;
+  static constexpr int kATile = TC_BM * kBK * 2;
+  static constexpr int kBTile = BN * kBK * 2;
+  static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;
   static constexpr int kSmemBytes = kStages * kStageBytes + 256 /*barriers*/ + 1024 /*align slack*/;
 };
 
@@ -225,16 +229,20 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
                   int M, int N, int K, TcEpilogue ep) {
   cn_pdl_trigger();                                 // PDL: the successor may be scheduled while this grid runs
   constexpr int TC_STAGES = TcCfg<BN>::kStages;
+  constexpr int BK = TcCfg<BN>::kBK;
+  constexpr int SW = TcCfg<BN>::kSwizzle;
+  constexpr int TC_A_TILE_BYTES = TcCfg<BN>::kATile;
   constexpr int TC_B_TILE_BYTES = TcCfg<BN>::kBTile;
   constexpr int TC_STAGE_BYTES = TcCfg<BN>::kStageBytes;
+  static_assert(!PROMOTE || BK == 64, "PROMOTE sums 64-wide k-blocks");
   extern __shared__ uint8_t tc_smem_raw[];
   const uint32_t raw = tc::smem_u32(tc_smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t base = (raw + 1023u) & ~1023u;                 // swizzled tiles need 1024-byte alignment
   const uint32_t bar_base = base + TC_STAGES * TC_STAGE_BYTES;  // barriers after the operand ring
   const uint32_t bar_full = bar_base, bar_empty = bar_base + 64;   // full[s] = +8 s ; empty[s] = +64 + 8 s
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int num_kb = K / TC_BK;
+  const int num_kb = K / BK;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; ++s) {
@@ -278,10 +286,10 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
           const uint32_t full = bar_full + 8 * s;
           tc::mbar_expect_tx(full, TC_STAGE_BYTES);
           const uint32_t st = base + s * TC_STAGE_BYTES;
-          tc::tma_load_2d(st, &map_ahi, full, kb * TC_BK, m0);
-          tc::tma_load_2d(st + TC_A_TILE_BYTES, &map_alo, full, kb * TC_BK, m0);
-          tc::tma_load_2d(st + 2 * TC_A_TILE_BYTES, &map_bhi, full, kb * TC_BK, n0);
-          tc::tma_load_2d(st + 2 * TC_A_TILE_BYTES + TC_B_TILE_BYTES, &map_blo, full, kb * TC_BK, n0);
+          tc::tma_load_2d(st, &map_ahi, full, kb * BK, m0);
+          tc::tma_load_2d(st + TC_A_TILE_BYTES, &map_alo, full, kb * BK, m0);
+          tc::tma_load_2d(st + 2 * TC_A_TILE_BYTES, &map_bhi, full, kb * BK, n0);
+          tc::tma_load_2d(st + 2 * TC_A_TILE_BYTES + TC_B_TILE_BYTES, &map_blo, full, kb * BK, n0);
         }
       }
     }
@@ -316,10 +324,10 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
       tc::fence_regs(acc);
       tc::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < TC_BK / 16; ++k) {
+      for (int k = 0; k < BK / 16; ++k) {
         const uint32_t koff = k * 32;                             // 16 fp16 = 32 bytes inside the swizzle atom
-        const uint64_t dah = tc::make_desc<128>(a_hi + koff), dal = tc::make_desc<128>(a_lo + koff);
-        const uint64_t dbh = tc::make_desc<128>(b_hi + koff), dbl = tc::make_desc<128>(b_lo + koff);
+        const uint64_t dah = tc::make_desc<SW>(a_hi + koff), dal = tc::make_desc<SW>(a_lo + koff);
+        const uint64_t dbh = tc::make_desc<SW>(b_hi + koff), dbl = tc::make_desc<SW>(b_lo + koff);
         const bool first = k == 0 && (PROMOTE || kb == kb0);      // the MMA that starts a new sum overwrites acc
         tc::wgmma_f16<BN>(acc, dah, dbh, first ? 0u : 1u);
         tc::wgmma_f16<BN>(acc, dah, dbl, 1u);

@@ -607,16 +607,17 @@ void* cn_gst_tc_create(int N, int H, int P, float thr, float pen, int device, co
     const int r = rows[tw[i].idx], k = cols[tw[i].idx];
     const float* d = nullptr;
     rc = gt_upload(ctx, &d, host[tw[i].idx], (size_t)r * k);
-    if (!rc) rc = tc_alloc(ctx, *tw[i].t, r, k, r == 256 ? 256 : 64);        // the 256-wide gate GEMMs use BN = 256 tiles
+    const int bn = r == 256 ? 256 : 64;                                       // the 256-wide gate GEMMs use BN = 256 tiles
+    if (!rc) rc = tc_alloc(ctx, *tw[i].t, r, k, bn, tc_box_k(bn));
     if (!rc) split16(ctx, 0, d, 64.0f, tw[i].t->hi, tw[i].t->lo, (size_t)r * k);
   }
   const size_t R = (size_t)N * GT_T * H, Rd = (size_t)N * H;
-  if (!rc) rc = tc_alloc(ctx, g->tX, (int)R, 64, TC_BM);
-  if (!rc) rc = tc_alloc(ctx, g->tA, (int)R, 64, TC_BM);
-  if (!rc) rc = tc_alloc(ctx, g->tY, (int)R, 64, TC_BM);
-  if (!rc) rc = tc_alloc(ctx, g->tF, (int)R, 128, TC_BM);
-  if (!rc) rc = tc_alloc(ctx, g->tXS, (int)R, 64, TC_BM);
-  if (!rc) rc = tc_alloc(ctx, g->tHd, (int)Rd, 64, TC_BM);
+  if (!rc) rc = tc_alloc(ctx, g->tX, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tA, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tY, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tF, (int)R, 128, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tXS, (int)R, 64, TC_BM, tc_box_k(256));     // A of the BN = 256 gate GEMMs
+  if (!rc) rc = tc_alloc(ctx, g->tHd, (int)Rd, 64, TC_BM, tc_box_k(256));
 #define GA(name, count) if (!rc) rc = palloc(ctx, &g->name, (count))
   GA(X0, R * 64); GA(QKV, R * 192); GA(O, R * 64); GA(X1, R * 64); GA(GX, R * 256); GA(GH, Rd * 256); GA(rowm, R); GA(fp, Rd);
   GA(pos_last, Rd * 2); GA(h32, Rd * 64); GA(c32, Rd * 64); GA(mu_cum, Rd * 2); GA(xin, Rd * 2); GA(pred, Rd * GT_T * 2);

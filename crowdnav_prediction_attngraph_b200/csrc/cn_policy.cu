@@ -29,6 +29,7 @@ struct TcMat {
   __half *hi = nullptr, *lo = nullptr;
   CUtensorMap mh, ml;
   int pitch = 0;
+  int box_k = 0;   // k width of the TMA box of mh / ml: the k-block of the GEMM instance that reads it
 };
 
 struct cn_policy {
@@ -146,20 +147,24 @@ int halloc16(cn_policy* p, __half** ptr, size_t count) {
   return rc;
 }
 
-// allocate a split matrix [rows, K] and build its maps (box_rows = 128 for A operands, BN for B operands)
-int tc_alloc(cn_policy* p, TcMat& t, int rows, int K, int box_rows) {
+// k width of the TMA boxes of the GEMM instance with B-tile rows bn (32 for BN = 256, 64 for BN = 64)
+int tc_box_k(int bn) { return bn == 256 ? TcCfg<256>::kBK : TcCfg<64>::kBK; }
+
+// allocate a split matrix [rows, K] and build its maps (box_rows = 128 for A operands, BN for B operands;
+// box_k = tc_box_k(BN) of the instance that reads it)
+int tc_alloc(cn_policy* p, TcMat& t, int rows, int K, int box_rows, int box_k) {
   int rc = halloc16(p, &t.hi, (size_t)rows * K);
   if (!rc) rc = halloc16(p, &t.lo, (size_t)rows * K);
-  t.pitch = K;
-  if (!rc) rc = make_map(&t.mh, t.hi, rows, K, box_rows, K);
-  if (!rc) rc = make_map(&t.ml, t.lo, rows, K, box_rows, K);
+  t.pitch = K; t.box_k = box_k;
+  if (!rc) rc = make_map(&t.mh, t.hi, rows, K, box_rows, K, box_k);
+  if (!rc) rc = make_map(&t.ml, t.lo, rows, K, box_rows, K, box_k);
   return rc;
 }
-// view of columns [col0, col0 + K) of an existing split matrix
+// view of columns [col0, col0 + K) of an existing split matrix (same box width as the source)
 int tc_view(TcMat& v, const TcMat& src, int col0, int rows, int K, int box_rows) {
-  v.hi = src.hi + col0; v.lo = src.lo + col0; v.pitch = src.pitch;
-  int rc = make_map(&v.mh, v.hi, rows, K, box_rows, src.pitch);
-  if (!rc) rc = make_map(&v.ml, v.lo, rows, K, box_rows, src.pitch);
+  v.hi = src.hi + col0; v.lo = src.lo + col0; v.pitch = src.pitch; v.box_k = src.box_k;
+  int rc = make_map(&v.mh, v.hi, rows, K, box_rows, src.pitch, src.box_k);
+  if (!rc) rc = make_map(&v.ml, v.lo, rows, K, box_rows, src.pitch, src.box_k);
   return rc;
 }
 
@@ -212,6 +217,15 @@ void gemm_tc(cn_policy* p, cudaStream_t st, const TcMat& A, const TcMat& B, int 
   {
     static const int nostore = (getenv("CN_DBG_NOSTORE") && getenv("CN_DBG_NOSTORE")[0] == '1') ? 1 : 0;
     ep.dbg_nostore = nostore;
+  }
+  // the operand maps must have the box width this instance loads, or its barriers would wait for bytes that never come
+  if (A.box_k != tc_box_k(bn) || B.box_k != tc_box_k(bn)) {
+    if (!p->launch_error) {
+      p->launch_error = true;
+      cn_set_error("gemm_tc in stage '%s': operand boxes %d / %d wide, the BN = %d instance loads %d",
+                   p->cur_stage ? p->cur_stage : "?", A.box_k, B.box_k, bn, tc_box_k(bn));
+    }
+    return;
   }
   // persistent: one CTA per SM at most; tiles beyond the device-side row count are never touched
   const int tiles = (N / bn) * ((M + TC_BM - 1) / TC_BM);
@@ -341,17 +355,18 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
 #undef WS
   if (!rc && cfg->gemm_mode == 1) {
     // A operands: box rows = 128 (TC_BM)
-    rc = tc_alloc(p, p->tE1, Mi, 128, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tE2, Mi, 512, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tAo, Mi, 512, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tRs, Ni, 256, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tT1, Ni, 128, TC_BM);                 // [enc | te] then [enc | emb]
+    // per-human rows feed the BN = 256 instance, per-environment rows the BN = 64 one
+    rc = tc_alloc(p, p->tE1, Mi, 128, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(p, p->tE2, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(p, p->tAo, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(p, p->tRs, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(p, p->tT1, Ni, 128, TC_BM, tc_box_k(64));   // [enc | te] then [enc | emb]
     if (!rc) rc = tc_view(p->tTe, p->tT1, 64, Ni, 64, TC_BM);           // te = columns 64..127
-    if (!rc) rc = tc_alloc(p, p->tWv, Ni, 256, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tH0, Ni, 128, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tH1, Ni, 128, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tOut, Ni, 256, TC_BM);
-    if (!rc) rc = tc_alloc(p, p->tAc1, Ni, 512, TC_BM);
+    if (!rc) rc = tc_alloc(p, p->tWv, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(p, p->tH0, Ni, 128, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(p, p->tH1, Ni, 128, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(p, p->tOut, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(p, p->tAc1, Ni, 512, TC_BM, tc_box_k(64));
     if (!rc) rc = tc_view(p->tA1, p->tAc1, 0, Ni, 256, TC_BM);          // actor.0 half
     if (!rc) rc = tc_view(p->tC1, p->tAc1, 256, Ni, 256, TC_BM);        // critic.0 half
     if (!rc) rc = tc_set_attrs();
@@ -505,7 +520,7 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
         {p->Wih, &p->tWih, 384, 128, 64},   {p->Whh, &p->tWhh, 384, 128, 64},     {p->Wo, &p->tWo, 256, 128, 64},
         {p->Wac1, &p->tWac1, 512, 256, 64}, {p->Wa2, &p->tWa2, 256, 256, 64},     {p->Wc2, &p->tWc2, 256, 256, 64}};
     for (auto& t : tw) {
-      rc = tc_alloc(p, *t.t, t.rows, t.k, t.bn);
+      rc = tc_alloc(p, *t.t, t.rows, t.k, t.bn, tc_box_k(t.bn));
       if (rc) return rc;
       split16(p, st, t.src, 64.0f, t.t->hi, t.t->lo, (size_t)t.rows * t.k);
     }
@@ -514,7 +529,7 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
       float* wh = nullptr;
       rc = palloc(p, &wh, (size_t)1536 * 512);
       if (!rc) rc = palloc(p, &p->bqkvH, 1536);
-      if (!rc) rc = tc_alloc(p, p->tWqkvH, 1536, 512, QA_BN);
+      if (!rc) rc = tc_alloc(p, p->tWqkvH, 1536, 512, QA_BN, QA_BK);
       if (!rc) rc = make_map(&p->qa_bh, p->tWqkvH.hi, 1536, 512, QA_BN, 512, QA_BK);
       if (!rc) rc = make_map(&p->qa_bl, p->tWqkvH.lo, 1536, 512, QA_BN, 512, QA_BK);
       if (!rc) rc = make_map(&p->qa_ah, p->tE2.hi, p->M, 512, TC_BM, 512, QA_BK);
@@ -703,9 +718,9 @@ int cn_internal_gemm_tc_ex(const float* dA, const float* dW, const float* dbias,
   tmp.num_sms = 132; tmp.qkv_chunks = 1; tmp.launch_error = false; tmp.pdl = false;
   cudaDeviceGetAttribute(&tmp.num_sms, cudaDevAttrMultiProcessorCount, 0);
   TcMat Af, A, B;
-  int rc = tc_alloc(&tmp, Af, M, a_pitch, TC_BM);
+  int rc = tc_alloc(&tmp, Af, M, a_pitch, TC_BM, tc_box_k(bn));
   if (!rc) rc = tc_view(A, Af, a_col0, M, K, TC_BM);
-  if (!rc) rc = tc_alloc(&tmp, B, N, K, bn);
+  if (!rc) rc = tc_alloc(&tmp, B, N, K, bn, tc_box_k(bn));
   if (!rc) rc = tc_set_attrs();
   if (!rc) {
     split16(&tmp, 0, dA, 1.0f, Af.hi, Af.lo, (size_t)M * a_pitch);
