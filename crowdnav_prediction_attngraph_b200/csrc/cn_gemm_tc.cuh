@@ -17,7 +17,10 @@
 // MMA time instead of half of it; each output element still sees the same wgmma instructions in the same order.
 // Warp groups: 0 = TMA producer (one thread), 1 and 2 = consumers: each issues wgmma.m64nBNk16 for 64 rows of the
 // tile, keeps that 64 x BN fp32 accumulator in registers and runs the epilogue (bias, activation, stores) straight
-// from them.
+// from them.  The activation and the output kind are template parameters of the non-PROMOTE instances: an epilogue
+// that chose them at run time inlined every path into each of the 64 unrolled column groups of BN = 256 (20 680
+// instructions, ~330 KB of code walked on every tile), and that epilogue, not the MMAs, set the time of a tile (QKV:
+// 31 of 46 us; now 9 of 24 us, DESIGN.md 3.2).  The QKV instance is now 1 048 instructions.
 //
 // PROMOTE (the PPO update's GEMMs, which must be fp32-equivalent): the tensor core sums each 64-wide k-block on its own
 // and the CUDA cores add the block sums into a second register accumulator with IEEE round-to-nearest.  wgmma's fp32
@@ -64,7 +67,20 @@ struct TcEpilogue {
   int ksplit;                 // > 1 (PROMOTE only): the K range is cut into `ksplit` slices, every slice is its own tile and ADDS its
                               // partial product into a zero-initialised fp32 C with atomic adds (bias from slice 0
                               // only, no activation): wgrad has K = #rows (hundreds of thousands) and a tiny output
+#ifdef CN_GEMM_TRACE
+  unsigned long long* trace;  // [gridDim.x][trace_cap][5] per-tile records (tools/gemm_tile_trace.py)
+  int trace_cap;
+#endif
 };
+
+// Output kinds of the non-PROMOTE instances (template parameter OUT): fp32 C, split fp16 (hi, lo), or both
+enum { TC_OUT_F32 = 1, TC_OUT_F16 = 2, TC_OUT_BOTH = 3 };
+
+#ifdef CN_GEMM_TRACE
+#define TC_TRACE(...) __VA_ARGS__
+#else
+#define TC_TRACE(...)
+#endif
 
 namespace tc {
 
@@ -90,6 +106,27 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   } while (!ok);
 }
+#ifdef CN_GEMM_TRACE
+// mbar_wait that returns the number of failed polls
+__device__ __forceinline__ uint32_t mbar_wait_polls(uint32_t bar, uint32_t parity) {
+  uint32_t ok, n = 0;
+  while (true) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+    if (ok) return n;
+    ++n;
+  }
+}
+__device__ __forceinline__ uint64_t globaltimer() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#endif
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -218,11 +255,52 @@ __device__ __forceinline__ uint32_t split_pair_hi(float x0, float x1, uint32_t* 
 
 }  // namespace tc
 
+// Epilogue of the non-PROMOTE instances: scale, bias, activation and stores straight from the 64 x BN accumulator of
+// one consumer warp group (this thread: rows r0, r0 + 8; columns 8 g + cq, + 1).  The activation (CN_ACT_*) and the
+// output kind (TC_OUT_*) are compile-time, so each instance holds only the code it runs; the [act_lo, act_hi) window
+// is a per-column select.  Rows at or past m_ext (the output's extent) are not stored.
+template <int BN, int ACT, int OUT>
+__device__ __forceinline__ void tc_epilogue_store(const float (&acc)[BN / 2], const TcEpilogue& ep, float inv_scale,
+                                                  int n0, int r0, int cq, int m_ext) {
+  static_assert(ACT >= 0 && ACT <= 2 && OUT >= TC_OUT_F32 && OUT <= TC_OUT_BOTH, "epilogue kind");
+  const int row_end = ep.dbg_nostore ? 0 : m_ext;       // CN_DBG_NOSTORE: all the arithmetic, no stores
+#pragma unroll
+  for (int g = 0; g < BN / 8; ++g) {
+    const int col = n0 + 8 * g + cq;
+    const float b0 = ep.bias ? __ldg(ep.bias + col) : 0.0f, b1 = ep.bias ? __ldg(ep.bias + col + 1) : 0.0f;
+    const bool w0 = col >= ep.act_lo && col < ep.act_hi, w1 = col + 1 >= ep.act_lo && col + 1 < ep.act_hi;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      float v0 = fmaf(acc[4 * g + 2 * h], inv_scale, b0), v1 = fmaf(acc[4 * g + 2 * h + 1], inv_scale, b1);
+      if constexpr (ACT == 1) {
+        v0 = w0 ? fmaxf(v0, 0.0f) : v0; v1 = w1 ? fmaxf(v1, 0.0f) : v1;
+      } else if constexpr (ACT == 2) {
+        if (w0) v0 = tc::fast_tanh(v0);
+        if (w1) v1 = tc::fast_tanh(v1);
+      }
+      if (row >= row_end) continue;
+      if constexpr ((OUT & TC_OUT_F32) != 0) {
+        *reinterpret_cast<float2*>(ep.c32 + (size_t)row * ep.ldc + col) = make_float2(v0, v1);
+      }
+      if constexpr ((OUT & TC_OUT_F16) != 0) {
+        uint32_t lo;
+        const uint32_t hi = tc::split_pair_hi(v0, v1, &lo);
+        const size_t o = (size_t)row * ep.ldh + col;
+        *reinterpret_cast<uint32_t*>(ep.out_hi + o) = hi;
+        *reinterpret_cast<uint32_t*>(ep.out_lo + o) = lo;
+      }
+    }
+  }
+}
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, blockIdx.x + grid, ...
 // (n fastest, so CTAs running at the same time share A rows in L2).  The row count may live on the
 // device (ep.m_ptr, compacted human rows): no CTA is ever launched for an empty tile.  Rows are stored
 // up to M (the output's extent), columns up to N (a multiple of BN).
-template <int BN, bool PROMOTE = false>
+// ACT (CN_ACT_*) and OUT (TC_OUT_*) select the epilogue of the non-PROMOTE instances (tc_epilogue_store); the PROMOTE
+// instance keeps the run-time epilogue below (activation from ep.act, atomic adds with split-K) and ignores them.
+template <int BN, bool PROMOTE = false, int ACT = 0, int OUT = TC_OUT_F32>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
                   const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
@@ -304,10 +382,14 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
   const int wr = 16 * (warp & 3) + (lane >> 2);                   // first accumulator row of this thread in its half
   const int cq = 2 * (lane & 3);                                  // first accumulator column inside each 8-column group
   uint32_t it = 0;
+  // trace (CN_GEMM_TRACE builds only): consumer warp 0 records, per tile, the tile start, the first full-barrier pass,
+  // the main-loop end, the epilogue end (%globaltimer, ns) and its failed polls of the full barriers
+  TC_TRACE(const bool tr = ep.trace && warp == 4 && lane == 0; int tr_n = 0;)
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int mn = tile % n_mn, ks = tile / n_mn;
     const int m0 = m_lo + (mn / n_ntiles) * TC_BM, n0 = (mn % n_ntiles) * BN;
     const int kb0 = ks * kb_per, kb1 = (kb0 + kb_per < num_kb) ? kb0 + kb_per : num_kb;
+    TC_TRACE(const uint64_t t_tile = tc::globaltimer(); uint64_t t_first = 0; uint32_t polls = 0;)
     float acc[BN / 2];
     float sum[PROMOTE ? BN / 2 : 1];
     if constexpr (PROMOTE) {
@@ -317,7 +399,12 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
     uint32_t prev = 0;
     for (int kb = kb0; kb < kb1; ++kb, ++it) {
       const uint32_t s = it % TC_STAGES, ph = (it / TC_STAGES) & 1u;
+#ifdef CN_GEMM_TRACE
+      polls += tc::mbar_wait_polls(bar_full + 8 * s, ph);
+      if (kb == kb0) t_first = tc::globaltimer();
+#else
       tc::mbar_wait(bar_full + 8 * s, ph);                        // TMA bytes landed
+#endif
       const uint32_t st = base + s * TC_STAGE_BYTES;
       const uint32_t a_hi = st + half * (TC_A_TILE_BYTES / 2), a_lo = a_hi + TC_A_TILE_BYTES,
                      b_hi = st + 2 * TC_A_TILE_BYTES, b_lo = b_hi + TC_B_TILE_BYTES;
@@ -362,7 +449,18 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
       if (lane == 0) tc::mbar_arrive(bar_empty + 8 * prev);
     }
 
-    // ---- epilogue: scale, bias, activation, stores from the accumulator registers ----
+    TC_TRACE(const uint64_t t_loop = tc::globaltimer();)
+    if constexpr (!PROMOTE) {
+      tc_epilogue_store<BN, ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half + wr, cq, m_ext);
+      TC_TRACE(
+        if (tr && tr_n < ep.trace_cap) {
+          unsigned long long* rec = ep.trace + ((size_t)blockIdx.x * ep.trace_cap + tr_n) * 5;
+          rec[0] = t_tile; rec[1] = t_first; rec[2] = t_loop; rec[3] = tc::globaltimer(); rec[4] = polls;
+        }
+        ++tr_n;)
+      continue;
+    }
+    // ---- PROMOTE epilogue: scale, bias, activation, stores (atomic adds with split-K) from the accumulator ----
     // activation is uniform over the tile unless the [act_lo, act_hi) window cuts through it
     const bool act_full = ep.act_lo <= n0 && ep.act_hi >= n0 + BN;
     const bool act_none = ep.act == 0 || ep.act_hi <= n0 || ep.act_lo >= n0 + BN;

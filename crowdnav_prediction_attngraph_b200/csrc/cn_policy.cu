@@ -202,6 +202,25 @@ void split16(cn_policy* p, cudaStream_t st, const float* src, float scale, __hal
   p->launches += 1;
 }
 
+// the non-PROMOTE instance of cn_gemm_tc_kernel with B-tile rows BN, activation act (CN_ACT_*) and output kind out (TC_OUT_*)
+typedef void (*TcKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, TcEpilogue);
+template <int BN>
+TcKernel tc_kernel(int act, int out) {
+  static const TcKernel k[3][3] = {
+      {cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_F16>,
+       cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_BOTH>},
+      {cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_F16>,
+       cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_BOTH>},
+      {cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_F16>,
+       cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_BOTH>}};
+  return k[act][out - 1];
+}
+
+#ifdef CN_GEMM_TRACE
+unsigned long long* g_tc_trace = nullptr;   // per-tile trace buffer of every following gemm_tc launch (or null)
+int g_tc_trace_cap = 0;
+#endif
+
 // tensor-core GEMM launch: C = act((Ahi+Alo)(Bhi+Blo)^T / 64 + bias); bn = B tile rows (256 or 64)
 struct TcOut {
   float* c32 = nullptr; int ldc = 0;
@@ -227,23 +246,38 @@ void gemm_tc(cn_policy* p, cudaStream_t st, const TcMat& A, const TcMat& B, int 
     }
     return;
   }
+  const int out_kind = (o.c32 ? TC_OUT_F32 : 0) | (o.oh ? TC_OUT_F16 : 0);
+  if (act < CN_ACT_NONE || act > CN_ACT_TANH || !out_kind) {
+    if (!p->launch_error) {
+      p->launch_error = true;
+      cn_set_error("gemm_tc in stage '%s': activation %d / no output", p->cur_stage ? p->cur_stage : "?", act);
+    }
+    return;
+  }
+#ifdef CN_GEMM_TRACE
+  ep.trace = g_tc_trace; ep.trace_cap = g_tc_trace_cap;
+#endif
   // persistent: one CTA per SM at most; tiles beyond the device-side row count are never touched
   const int tiles = (N / bn) * ((M + TC_BM - 1) / TC_BM);
   dim3 grid(tiles < p->num_sms ? tiles : p->num_sms);
   if (bn == 256)
-    launch_k(p, cn_gemm_tc_kernel<256>, grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
+    launch_k(p, tc_kernel<256>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
   else
-    launch_k(p, cn_gemm_tc_kernel<64>, grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
+    launch_k(p, tc_kernel<64>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
 }
 TcOut out32(float* c, int ldc) { TcOut o; o.c32 = c; o.ldc = ldc; return o; }
 TcOut out16(const TcMat& t) { TcOut o; o.oh = t.hi; o.ol = t.lo; o.ldh = t.pitch; return o; }
 TcOut out_both(float* c, int ldc, const TcMat& t) { TcOut o = out16(t); o.c32 = c; o.ldc = ldc; return o; }
 
 int tc_set_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(cn_gemm_tc_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       TcCfg<256>::kSmemBytes);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(cn_gemm_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::kSmemBytes);
+  cudaError_t e = cudaSuccess;
+  for (int act = CN_ACT_NONE; act <= CN_ACT_TANH; ++act)
+    for (int out = TC_OUT_F32; out <= TC_OUT_BOTH; ++out) {
+      if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(tc_kernel<256>(act, out), cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<256>::kSmemBytes);
+      if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(tc_kernel<64>(act, out), cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::kSmemBytes);
+    }
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(cn_qkv_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QA_SMEM_BYTES);
   if (e != cudaSuccess) return cn_set_error("cudaFuncSetAttribute(tc): %s", cudaGetErrorString(e));
@@ -740,6 +774,15 @@ int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, fl
                         int bn) {
   return cn_internal_gemm_tc_ex(dA, dW, dbias, dC, M, N, K, act, bn, nullptr, nullptr, 0, 0, nullptr, nullptr, 0, 0, 0);
 }
+
+#ifdef CN_GEMM_TRACE
+// Traced builds only (tools/gemm_tile_trace.py): every following gemm_tc launch writes per-tile records
+// [gridDim.x][cap][5] (tile start, first full-barrier pass, main-loop end, epilogue end, failed polls) to dtrace.
+int cn_internal_gemm_trace(unsigned long long* dtrace, int cap) {
+  g_tc_trace = dtrace; g_tc_trace_cap = dtrace ? cap : 0;
+  return 0;
+}
+#endif
 
 // Internal test hook (not part of the public header): where one named workspace buffer of the policy forward lives,
 // so a test can read every stage's input and output back after cn_policy_act.  *kind = 0: fp32 at *ptr; 1: fp16
