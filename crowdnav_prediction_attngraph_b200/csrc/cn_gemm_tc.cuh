@@ -16,8 +16,9 @@
 // atom).  BN = 256: k-blocks of 32 fp16 (64-byte swizzle), so a slot is refilled after a quarter of the ring's
 // MMA time instead of half of it; each output element still sees the same wgmma instructions in the same order.
 // Warp groups: 0 = TMA producer (one thread), 1 and 2 = consumers: each issues wgmma.m64nBNk16 for 64 rows of the
-// tile, keeps that 64 x BN fp32 accumulator in registers and runs the epilogue (bias, activation, stores) straight
-// from them.  The activation and the output kind are template parameters of the non-PROMOTE instances: an epilogue
+// tile, keeps that 64 x BN fp32 accumulator in registers and runs the epilogue (bias, activation, stores) from them:
+// BN = 64 stores straight to global memory, BN = 256 stages boxes in shared memory and stores them with TMA while the
+// warp group goes on (tc_epilogue_tma).  The activation and the output kind are template parameters of the non-PROMOTE instances: an epilogue
 // that chose them at run time inlined every path into each of the 64 unrolled column groups of BN = 256 (20 680
 // instructions, ~330 KB of code walked on every tile), and that epilogue, not the MMAs, set the time of a tile (QKV:
 // 31 of 46 us; now 9 of 24 us, DESIGN.md 3.2).  The QKV instance is now 1 048 instructions.
@@ -45,7 +46,14 @@ struct TcCfg {
   static constexpr int kATile = TC_BM * kBK * 2;
   static constexpr int kBTile = BN * kBK * 2;
   static constexpr int kStageBytes = 2 * kATile + 2 * kBTile;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 256 /*barriers*/ + 1024 /*align slack*/;
+  // BN = 256: the epilogue stages its output in shared memory, in boxes of 64 rows x 128 bytes (32 fp32 or 64 fp16
+  // columns, 128-byte swizzle) that TMA stores; kStoreBoxes boxes per consumer warp group (tc_epilogue_tma).  Two boxes
+  // fit beside the 4-stage ring (230 656 B of the 232 448 B opt-in limit).  A 3-stage ring with four boxes measured the
+  // same for embed2 and qkv and 6 % slower for outproj_spatial, whose main loop then waits for operands (DESIGN.md 3.2).
+  static constexpr int kStoreBoxes = (BN >= 256) ? 2 : 0;
+  static constexpr int kBoxBytes = 64 * 128;
+  static constexpr int kStagingBytes = 2 * kStoreBoxes * kBoxBytes;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kStagingBytes + 256 /*barriers*/ + 1024 /*align slack*/;
 };
 
 struct TcEpilogue {
@@ -68,10 +76,18 @@ struct TcEpilogue {
                               // partial product into a zero-initialised fp32 C with atomic adds (bias from slice 0
                               // only, no activation): wgrad has K = #rows (hundreds of thousands) and a tiny output
 #ifdef CN_GEMM_TRACE
-  unsigned long long* trace;  // [gridDim.x][trace_cap][5] per-tile records (tools/gemm_tile_trace.py)
+  unsigned long long* trace;  // [gridDim.x][trace_cap][TC_TRACE_REC] per-tile records (tools/gemm_tile_trace.py)
   int trace_cap;
 #endif
 };
+
+#ifdef CN_GEMM_TRACE
+// per-tile trace record: tile start, first full-barrier pass, main-loop end, epilogue end (%globaltimer, ns; for
+// BN = 256 the moment the recording thread handed the tile's last box to TMA), failed polls of the full barriers;
+// BN = 256 only: staging-buffer waits that blocked, and the clock cycles spent in all staging-buffer waits
+#define TC_TRACE_REC 7
+#define TC_TRACE_WAIT_CLK 100     // a wait on a buffer that is already free returns well within this many cycles
+#endif
 
 // Output kinds of the non-PROMOTE instances (template parameter OUT): fp32 C, split fp16 (hi, lo), or both
 enum { TC_OUT_F32 = 1, TC_OUT_F16 = 2, TC_OUT_BOTH = 3 };
@@ -134,6 +150,23 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 }
 __device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// TMA store of one box from shared memory (bulk-group completion) and the bulk-group bookkeeping of the issuing thread
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy writes to shared memory -> visible to the async proxy (TMA) after the next barrier
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // K-major shared-memory matrix descriptor of wgmma (cute::GMMA::DescriptorSW128 / SW64) for a tile written by TMA
@@ -294,17 +327,144 @@ __device__ __forceinline__ void tc_epilogue_store(const float (&acc)[BN / 2], co
   }
 }
 
+// Staging buffers of tc_epilogue_tma.  Acquire: the issuing thread waits until at most PENDING of its box stores may
+// still be reading shared memory (so the buffers about to be written are free), then the warp group (named barrier
+// bar_id, 128 threads) goes on.  Release: every thread's writes are made visible to the async proxy before the
+// barrier after which the issuing thread hands the boxes to TMA.
+struct TcStaging {
+  uint32_t base;     // this warp group's kStoreBoxes boxes (1024-byte aligned)
+  uint32_t box;      // running box counter: box b is staged in buffer b % kStoreBoxes
+  bool leader;       // the warp group's thread that issues (and drains) the TMA stores
+  int bar_id;
+#ifdef CN_GEMM_TRACE
+  uint32_t waits;    // acquires that blocked (TC_TRACE_WAIT_CLK), and the cycles spent in all of them
+  uint64_t wait_clk;
+#endif
+  template <int PENDING>
+  __device__ __forceinline__ void acquire() {
+    if (leader) {
+#ifdef CN_GEMM_TRACE
+      const long long c0 = clock64();
+      tc::bulk_wait_read<PENDING>();
+      const long long d = clock64() - c0;
+      waits += d > TC_TRACE_WAIT_CLK ? 1u : 0u;
+      wait_clk += (uint64_t)d;
+#else
+      tc::bulk_wait_read<PENDING>();
+#endif
+    }
+    tc::named_bar_sync(bar_id, 128);
+  }
+  __device__ __forceinline__ void release() {
+    tc::fence_proxy_async_smem();
+    tc::named_bar_sync(bar_id, 128);
+  }
+  __device__ __forceinline__ uint32_t buf(uint32_t b) const { return base + (b % TcCfg<256>::kStoreBoxes) * TcCfg<256>::kBoxBytes; }
+};
+
+// Epilogue of the BN = 256 non-PROMOTE instances: the arithmetic of tc_epilogue_store (same operations, same order),
+// but the warp group's 64 x 256 result goes through shared memory.  Each box of 64 rows x 128 bytes (fp32: 32 columns;
+// split fp16: 64 columns of hi and, in a second box, of lo) is written in the 128-byte swizzle of the output maps: a
+// 16-byte chunk c of row r sits at chunk c ^ (r & 7), so the eight rows of a warp's store land in different banks.
+// One thread then stores the box with TMA and the warp group moves on without waiting for the global writes; the map's
+// row extent (the output's extent M) clips rows as `row < m_ext` does in tc_epilogue_store.  CN_DBG_NOSTORE: stage,
+// issue nothing.  This thread: rows wr, wr + 8 of the half starting at row m_half; columns 8 g + cq, + 1.
+template <int ACT, int OUT>
+__device__ __forceinline__ void tc_epilogue_tma(const float (&acc)[128], const TcEpilogue& ep, float inv_scale, int n0,
+                                                int m_half, int wr, int lane, TcStaging& sg, const CUtensorMap* map_c,
+                                                const CUtensorMap* map_oh, const CUtensorMap* map_ol) {
+  static_assert(ACT >= 0 && ACT <= 2 && OUT >= TC_OUT_F32 && OUT <= TC_OUT_BOTH, "epilogue kind");
+  constexpr int NB = TcCfg<256>::kStoreBoxes;
+  static_assert(NB >= 2 && (NB & (NB - 1)) == 0, "the split fp16 output stages hi and lo boxes together");
+  const int cq = 2 * (lane & 3);
+  const bool issue = sg.leader && !ep.dbg_nostore;
+  const uint32_t rsw = (uint32_t)(wr & 7);                        // swizzle phase of rows wr and wr + 8
+  const uint32_t row_off = (uint32_t)wr * 128u;
+  if constexpr ((OUT & TC_OUT_F32) != 0) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {                                 // box j: columns [32 j, 32 j + 32) of the tile
+      sg.acquire<NB - 1>();
+      const uint32_t b = sg.buf(sg.box) + row_off + 8u * (uint32_t)(lane & 1);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int g = 4 * j + q, col = n0 + 8 * g + cq;
+        const float b0 = ep.bias ? __ldg(ep.bias + col) : 0.0f, b1 = ep.bias ? __ldg(ep.bias + col + 1) : 0.0f;
+        const bool w0 = col >= ep.act_lo && col < ep.act_hi, w1 = col + 1 >= ep.act_lo && col + 1 < ep.act_hi;
+        const uint32_t chunk = (uint32_t)(2 * q + ((lane & 3) >> 1));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0 = fmaf(acc[4 * g + 2 * h], inv_scale, b0), v1 = fmaf(acc[4 * g + 2 * h + 1], inv_scale, b1);
+          if constexpr (ACT == 1) {
+            v0 = w0 ? fmaxf(v0, 0.0f) : v0; v1 = w1 ? fmaxf(v1, 0.0f) : v1;
+          } else if constexpr (ACT == 2) {
+            if (w0) v0 = tc::fast_tanh(v0);
+            if (w1) v1 = tc::fast_tanh(v1);
+          }
+          tc::st_shared_v2(b + 1024u * h + ((chunk ^ rsw) << 4), v0, v1);
+        }
+      }
+      sg.release();
+      if (issue) {
+        tc::tma_store_2d(map_c, sg.buf(sg.box), n0 + 32 * j, m_half);
+        tc::bulk_commit();
+      }
+      ++sg.box;
+    }
+  }
+  if constexpr ((OUT & TC_OUT_F16) != 0) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {                                 // boxes of hi and lo: columns [64 j, 64 j + 64)
+      sg.acquire<NB - 2>();
+      const uint32_t bh = sg.buf(sg.box) + row_off + 4u * (uint32_t)(lane & 3);
+      const uint32_t bl = sg.buf(sg.box + 1) + row_off + 4u * (uint32_t)(lane & 3);
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int g = 8 * j + q, col = n0 + 8 * g + cq;
+        const float b0 = ep.bias ? __ldg(ep.bias + col) : 0.0f, b1 = ep.bias ? __ldg(ep.bias + col + 1) : 0.0f;
+        const bool w0 = col >= ep.act_lo && col < ep.act_hi, w1 = col + 1 >= ep.act_lo && col + 1 < ep.act_hi;
+        const uint32_t sw_off = ((uint32_t)q ^ rsw) << 4;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float v0 = fmaf(acc[4 * g + 2 * h], inv_scale, b0), v1 = fmaf(acc[4 * g + 2 * h + 1], inv_scale, b1);
+          if constexpr (ACT == 1) {
+            v0 = w0 ? fmaxf(v0, 0.0f) : v0; v1 = w1 ? fmaxf(v1, 0.0f) : v1;
+          } else if constexpr (ACT == 2) {
+            if (w0) v0 = tc::fast_tanh(v0);
+            if (w1) v1 = tc::fast_tanh(v1);
+          }
+          uint32_t lo;
+          const uint32_t hi = tc::split_pair_hi(v0, v1, &lo);
+          tc::st_shared_b32(bh + 1024u * h + sw_off, hi);
+          tc::st_shared_b32(bl + 1024u * h + sw_off, lo);
+        }
+      }
+      sg.release();
+      if (issue) {
+        tc::tma_store_2d(map_oh, sg.buf(sg.box), n0 + 64 * j, m_half);
+        tc::bulk_commit();
+        tc::tma_store_2d(map_ol, sg.buf(sg.box + 1), n0 + 64 * j, m_half);
+        tc::bulk_commit();
+      }
+      sg.box += 2;
+    }
+  }
+}
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, blockIdx.x + grid, ...
 // (n fastest, so CTAs running at the same time share A rows in L2).  The row count may live on the
 // device (ep.m_ptr, compacted human rows): no CTA is ever launched for an empty tile.  Rows are stored
 // up to M (the output's extent), columns up to N (a multiple of BN).
-// ACT (CN_ACT_*) and OUT (TC_OUT_*) select the epilogue of the non-PROMOTE instances (tc_epilogue_store); the PROMOTE
-// instance keeps the run-time epilogue below (activation from ep.act, atomic adds with split-K) and ignores them.
+// ACT (CN_ACT_*) and OUT (TC_OUT_*) select the epilogue of the non-PROMOTE instances (tc_epilogue_tma for BN = 256,
+// tc_epilogue_store for BN = 64); the PROMOTE instance keeps the run-time epilogue below (activation from ep.act, atomic
+// adds with split-K) and ignores them.  map_c / map_oh / map_ol: TMA store maps of the fp32 and split fp16 outputs,
+// [M rows, N columns] with boxes of 64 rows x 128 bytes and the 128-byte swizzle; read by the BN = 256 non-PROMOTE
+// instances only (the others get unused placeholders).
 template <int BN, bool PROMOTE = false, int ACT = 0, int OUT = TC_OUT_F32>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
                   const __grid_constant__ CUtensorMap map_bhi, const __grid_constant__ CUtensorMap map_blo,
-                  int M, int N, int K, TcEpilogue ep) {
+                  int M, int N, int K, TcEpilogue ep, const __grid_constant__ CUtensorMap map_c,
+                  const __grid_constant__ CUtensorMap map_oh, const __grid_constant__ CUtensorMap map_ol) {
   cn_pdl_trigger();                                 // PDL: the successor may be scheduled while this grid runs
   constexpr int TC_STAGES = TcCfg<BN>::kStages;
   constexpr int BK = TcCfg<BN>::kBK;
@@ -312,11 +472,14 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
   constexpr int TC_A_TILE_BYTES = TcCfg<BN>::kATile;
   constexpr int TC_B_TILE_BYTES = TcCfg<BN>::kBTile;
   constexpr int TC_STAGE_BYTES = TcCfg<BN>::kStageBytes;
+  constexpr bool kTmaStore = !PROMOTE && BN == 256;
   static_assert(!PROMOTE || BK == 64, "PROMOTE sums 64-wide k-blocks");
+  static_assert(!kTmaStore || TcCfg<BN>::kStoreBoxes > 0, "BN = 256 stages its output");
   extern __shared__ uint8_t tc_smem_raw[];
   const uint32_t raw = tc::smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // swizzled tiles need 1024-byte alignment
-  const uint32_t bar_base = base + TC_STAGES * TC_STAGE_BYTES;  // barriers after the operand ring
+  const uint32_t staging = base + TC_STAGES * TC_STAGE_BYTES;   // BN = 256: output staging after the operand ring
+  const uint32_t bar_base = staging + TcCfg<BN>::kStagingBytes; // barriers after them
   const uint32_t bar_full = bar_base, bar_empty = bar_base + 64;   // full[s] = +8 s ; empty[s] = +64 + 8 s
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
@@ -332,6 +495,13 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_alo) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_bhi) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_blo) : "memory");
+    if constexpr (kTmaStore) {
+      if constexpr ((OUT & TC_OUT_F32) != 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
+      if constexpr ((OUT & TC_OUT_F16) != 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_oh) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_ol) : "memory");
+      }
+    }
   }
   __syncthreads();
   // PDL: everything above (barrier init, descriptor prefetch) overlaps the predecessor's tail;
@@ -382,8 +552,12 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
   const int wr = 16 * (warp & 3) + (lane >> 2);                   // first accumulator row of this thread in its half
   const int cq = 2 * (lane & 3);                                  // first accumulator column inside each 8-column group
   uint32_t it = 0;
-  // trace (CN_GEMM_TRACE builds only): consumer warp 0 records, per tile, the tile start, the first full-barrier pass,
-  // the main-loop end, the epilogue end (%globaltimer, ns) and its failed polls of the full barriers
+  TcStaging sg;                                                   // BN = 256: this warp group's output staging
+  sg.base = staging + half * TcCfg<BN>::kStoreBoxes * TcCfg<BN>::kBoxBytes;
+  sg.box = 0; sg.leader = (threadIdx.x & 127) == 0; sg.bar_id = wg;   // named barriers 1, 2 (0 = __syncthreads)
+  TC_TRACE(sg.waits = 0; sg.wait_clk = 0;)
+  // trace (CN_GEMM_TRACE builds only): consumer warp 0 (the issuing thread of warp group 1) records one
+  // TC_TRACE_REC record per tile
   TC_TRACE(const bool tr = ep.trace && warp == 4 && lane == 0; int tr_n = 0;)
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int mn = tile % n_mn, ks = tile / n_mn;
@@ -451,11 +625,17 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
 
     TC_TRACE(const uint64_t t_loop = tc::globaltimer();)
     if constexpr (!PROMOTE) {
-      tc_epilogue_store<BN, ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half + wr, cq, m_ext);
+      TC_TRACE(const uint32_t waits0 = sg.waits; const uint64_t clk0 = sg.wait_clk;)
+      if constexpr (kTmaStore) {
+        tc_epilogue_tma<ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half, wr, lane, sg, &map_c, &map_oh, &map_ol);
+      } else {
+        tc_epilogue_store<BN, ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half + wr, cq, m_ext);
+      }
       TC_TRACE(
         if (tr && tr_n < ep.trace_cap) {
-          unsigned long long* rec = ep.trace + ((size_t)blockIdx.x * ep.trace_cap + tr_n) * 5;
+          unsigned long long* rec = ep.trace + ((size_t)blockIdx.x * ep.trace_cap + tr_n) * TC_TRACE_REC;
           rec[0] = t_tile; rec[1] = t_first; rec[2] = t_loop; rec[3] = tc::globaltimer(); rec[4] = polls;
+          rec[5] = sg.waits - waits0; rec[6] = sg.wait_clk - clk0;
         }
         ++tr_n;)
       continue;
@@ -502,6 +682,11 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
         }
       }
     }
+  }
+  // BN = 256: the box stores must have completed before the CTA exits.  Its shared memory is released then, and a
+  // dependent launch (griddepcontrol.wait after this grid) reads the output, visible only once the writes are done.
+  if constexpr (kTmaStore) {
+    if (sg.leader) tc::bulk_wait_all();
   }
 }
 

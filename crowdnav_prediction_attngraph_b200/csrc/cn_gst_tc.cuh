@@ -564,6 +564,7 @@ struct GstTc {
   TcMat tWin, tWout, tW1, tW2, tWih, tWhh;                   // weights (x 2^6, fp16 hi/lo)
   TcMat tX, tA, tY, tF, tXS, tHd;                            // activations (fp16 hi/lo A operands)
   float *X0, *QKV, *O, *X1, *GX, *GH, *rowm, *fp, *pos_last, *h32, *c32, *mu_cum, *xin, *pred;
+  TcStoreMap GX_R, GX_Rd, GH_Rd;                             // store maps of the BN = 256 gate GEMMs' outputs, per row extent
   // compact path (cn_gst_tcc_step): only rows whose mask is 1 are computed
   float* inp;                                                // [R, 2] masked input displacement of every (env, frame, human) row
   int *cidx, *crow, *gcount, *gstart, *ecount, *estart, *drow, *counts;   // compaction maps (see gtc_* kernels)
@@ -623,6 +624,10 @@ void* cn_gst_tc_create(int N, int H, int P, float thr, float pen, int device, co
   GA(pos_last, Rd * 2); GA(h32, Rd * 64); GA(c32, Rd * 64); GA(mu_cum, Rd * 2); GA(xin, Rd * 2); GA(pred, Rd * GT_T * 2);
   GA(inp, R * 2);
 #undef GA
+  // the encoder runs over all R observation rows and over the Rd rows of the newest frame: one GX map per row extent
+  if (!rc) rc = make_store_map(&g->GX_R, g->GX, 4, (int)R, 256, 256);
+  if (!rc) rc = make_store_map(&g->GX_Rd, g->GX, 4, (int)Rd, 256, 256);
+  if (!rc) rc = make_store_map(&g->GH_Rd, g->GH, 4, (int)Rd, 256, 256);
 #define GI(name, count) if (!rc) { float* q_ = nullptr; rc = palloc(ctx, &q_, (count)); g->name = reinterpret_cast<int*>(q_); }
   GI(cidx, R); GI(crow, R); GI(gcount, (size_t)N * GT_T); GI(gstart, (size_t)N * GT_T + 1); GI(ecount, N); GI(estart, N + 1);
   GI(drow, Rd); GI(counts, 4);
@@ -658,14 +663,14 @@ int cn_gst_tc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newest
     gemm_tc(p, st, g->tF, g->tW2, rows, 64, 128, 64, g->w.b2, CN_ACT_NONE, out32(g->O, 64));
     launch_k(p, gt_res_mask_kernel, dim3((unsigned)(((size_t)rows * 64 + 255) / 256)), dim3(256), 0, st, (size_t)rows * 64, g->X1, g->O,
              rowm, g->tXS.hi, g->tXS.lo);
-    gemm_tc(p, st, g->tXS, g->tWih, rows, 256, 64, 256, g->w.bih, CN_ACT_NONE, out32(g->GX, 256));
+    gemm_tc(p, st, g->tXS, g->tWih, rows, 256, 64, 256, g->w.bih, CN_ACT_NONE, out32(g->GX, 256, rows == R ? &g->GX_R : &g->GX_Rd));
   };
   launch_k(p, gt_prep_kernel, warps(R), dim3(256), 0, st, g->w, N, H, ring_pos, ring_mask, newest, robot, sp2, vis, g->X0, g->tX.hi,
            g->tX.lo, g->rowm, g->fp, g->pos_last, g->h32, g->tHd.hi, g->tHd.lo, g->c32, g->mu_cum);
   encoder(R, g->rowm);
   const unsigned cell_grid = (unsigned)((Rd * 64 + 255) / 256);
   for (int t = 0; t < GT_T; ++t) {
-    gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256));
+    gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd));
     launch_k(p, gt_cell_kernel, dim3(cell_grid), dim3(256), 0, st, N, H, g->GX, GT_T * H, t * H, g->GH, (const float*)nullptr, g->h32,
              g->c32, g->tHd.hi, g->tHd.lo);
   }
@@ -674,7 +679,7 @@ int cn_gst_tc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newest
     if (tt > 0) {
       launch_k(p, gt_embed_kernel, warps(Rd), dim3(256), 0, st, g->w, Rd, g->xin, g->fp, g->X0, g->tX.hi, g->tX.lo);
       encoder(Rd, g->fp);
-      gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256));
+      gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd));
       launch_k(p, gt_cell_kernel, dim3(cell_grid), dim3(256), 0, st, N, H, g->GX, H, 0, g->GH, g->fp, g->h32, g->c32, g->tHd.hi,
                g->tHd.lo);
     }
@@ -708,7 +713,8 @@ int cn_gst_tcc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newes
     gemm_tc(p, st, g->tY, g->tW1, maxrows, 128, 64, 64, g->w.b1, CN_ACT_RELU, out16(g->tF), cnt);
     gemm_tc(p, st, g->tF, g->tW2, maxrows, 64, 128, 64, g->w.b2, CN_ACT_NONE, out32(g->O, 64), cnt);
     launch_k(p, gtc_res_kernel, rows_grid, dim3(256), 0, st, cnt, g->X1, g->O, g->tXS.hi, g->tXS.lo);
-    gemm_tc(p, st, g->tXS, g->tWih, maxrows, 256, 64, 256, g->w.bih, CN_ACT_NONE, out32(g->GX, 256), cnt);
+    gemm_tc(p, st, g->tXS, g->tWih, maxrows, 256, 64, 256, g->w.bih, CN_ACT_NONE,
+            out32(g->GX, 256, maxrows == R ? &g->GX_R : &g->GX_Rd), cnt);
   };
   launch_k(p, gtc_prep_kernel, grp_grid, dim3(GTC_WARPS * 32), 0, st, N, H, ring_pos, ring_mask, newest, robot, sp2, vis, g->rowm, g->inp,
            g->gcount, g->ecount, g->fp, g->pos_last);
@@ -720,7 +726,7 @@ int cn_gst_tcc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newes
   // LSTM over the 5 observed frames, humans visible now only (h0 = c0 = 0: frame 0 has no recurrent GEMM, its
   // hidden-state gate term is b_hh)
   for (int t = 0; t < GT_T; ++t) {
-    if (t > 0) gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256), cntD);
+    if (t > 0) gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
     launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, t, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
              g->c32, g->tHd.hi, g->tHd.lo);
   }
@@ -728,7 +734,7 @@ int cn_gst_tcc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newes
     if (tt > 0) {
       launch_k(p, gtc_embed_kernel, rows_grid, dim3(256), 0, st, g->w, cntD, (const int*)nullptr, g->xin, g->X0, g->tX.hi, g->tX.lo);
       encoder(Rd, cntD, N, g->estart);
-      gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256), cntD);
+      gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
       launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, -1, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
                g->c32, g->tHd.hi, g->tHd.lo);
     }

@@ -24,12 +24,21 @@
 #include "cn_gemm_tc.cuh"
 #include "cn_qkv_attn.cuh"
 
+// TMA store map of an output of the BN = 256 GEMM instances: [rows, cols], boxes of 64 rows x 128 bytes, 128-byte
+// swizzle (cn_gemm_tc.cuh, tc_epilogue_tma).  rows = 0: no map (TMA needs a 16-byte-aligned base and a row pitch that
+// is a multiple of 16 bytes).
+struct TcStoreMap {
+  CUtensorMap map;
+  int rows = 0, cols = 0;
+};
+
 // A split-fp16 matrix [rows, K] (row pitch `pitch` elements) and its TMA descriptors.
 struct TcMat {
   __half *hi = nullptr, *lo = nullptr;
   CUtensorMap mh, ml;
   int pitch = 0;
   int box_k = 0;   // k width of the TMA box of mh / ml: the k-block of the GEMM instance that reads it
+  TcStoreMap sh, sl;   // store maps of hi / lo, for a BN = 256 GEMM that writes this matrix
 };
 
 struct cn_policy {
@@ -76,6 +85,7 @@ struct cn_policy {
   // workspace
   int *row_start, *row_env, *mc;
   float *x16, *e1, *e2, *qkv, *ao, *sout, *xr, *rs, *t1, *u, *wv, *h0, *gi, *gh, *outb, *ac1, *a2, *c2;
+  TcStoreMap qkv_st, sout_st;   // store maps of the fp32 outputs of the BN = 256 GEMMs (gemm_mode 1)
 };
 
 namespace {
@@ -150,6 +160,35 @@ int halloc16(cn_policy* p, __half** ptr, size_t count) {
 // k width of the TMA boxes of the GEMM instance with B-tile rows bn (32 for BN = 256, 64 for BN = 64)
 int tc_box_k(int bn) { return bn == 256 ? TcCfg<256>::kBK : TcCfg<64>::kBK; }
 
+// TMA can store a box into a matrix with this base and row pitch (bytes)
+bool tma_store_ok(const void* ptr, size_t pitch_bytes) { return ((uintptr_t)ptr % 16) == 0 && pitch_bytes % 16 == 0; }
+
+// store map of a BN = 256 output: fp32 (esize 4) or fp16 (esize 2) [rows, cols], row pitch `pitch` elements
+int make_store_map(TcStoreMap* s, const void* ptr, int esize, int rows, int cols, int pitch) {
+  s->rows = s->cols = 0;
+  if (!tma_store_ok(ptr, (size_t)pitch * esize))
+    return cn_set_error("TMA store map: base %p / row pitch %d B not 16-byte aligned", ptr, pitch * esize);
+  EncodeFn enc = get_encode();
+  if (!enc) return cn_set_error("cuTensorMapEncodeTiled entry point not available");
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)pitch * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(&s->map, esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
+                   const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return cn_set_error("cuTensorMapEncodeTiled(store) failed (%d) rows=%d cols=%d", (int)r, rows, cols);
+  s->rows = rows; s->cols = cols;
+  return 0;
+}
+// store maps of the hi / lo halves of a split matrix (left empty where TMA cannot store: an unaligned column view)
+int tc_store_maps(TcMat& t, int rows, int K) {
+  if (!tma_store_ok(t.hi, (size_t)t.pitch * 2) || !tma_store_ok(t.lo, (size_t)t.pitch * 2)) return 0;
+  int rc = make_store_map(&t.sh, t.hi, 2, rows, K, t.pitch);
+  if (!rc) rc = make_store_map(&t.sl, t.lo, 2, rows, K, t.pitch);
+  return rc;
+}
+
 // allocate a split matrix [rows, K] and build its maps (box_rows = 128 for A operands, BN for B operands;
 // box_k = tc_box_k(BN) of the instance that reads it)
 int tc_alloc(cn_policy* p, TcMat& t, int rows, int K, int box_rows, int box_k) {
@@ -158,6 +197,7 @@ int tc_alloc(cn_policy* p, TcMat& t, int rows, int K, int box_rows, int box_k) {
   t.pitch = K; t.box_k = box_k;
   if (!rc) rc = make_map(&t.mh, t.hi, rows, K, box_rows, K, box_k);
   if (!rc) rc = make_map(&t.ml, t.lo, rows, K, box_rows, K, box_k);
+  if (!rc) rc = tc_store_maps(t, rows, K);
   return rc;
 }
 // view of columns [col0, col0 + K) of an existing split matrix (same box width as the source)
@@ -165,6 +205,7 @@ int tc_view(TcMat& v, const TcMat& src, int col0, int rows, int K, int box_rows)
   v.hi = src.hi + col0; v.lo = src.lo + col0; v.pitch = src.pitch; v.box_k = src.box_k;
   int rc = make_map(&v.mh, v.hi, rows, K, box_rows, src.pitch, src.box_k);
   if (!rc) rc = make_map(&v.ml, v.lo, rows, K, box_rows, src.pitch, src.box_k);
+  if (!rc) rc = tc_store_maps(v, rows, K);
   return rc;
 }
 
@@ -203,7 +244,8 @@ void split16(cn_policy* p, cudaStream_t st, const float* src, float scale, __hal
 }
 
 // the non-PROMOTE instance of cn_gemm_tc_kernel with B-tile rows BN, activation act (CN_ACT_*) and output kind out (TC_OUT_*)
-typedef void (*TcKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, TcEpilogue);
+typedef void (*TcKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, TcEpilogue, CUtensorMap,
+                         CUtensorMap, CUtensorMap);
 template <int BN>
 TcKernel tc_kernel(int act, int out) {
   static const TcKernel k[3][3] = {
@@ -221,10 +263,13 @@ unsigned long long* g_tc_trace = nullptr;   // per-tile trace buffer of every fo
 int g_tc_trace_cap = 0;
 #endif
 
-// tensor-core GEMM launch: C = act((Ahi+Alo)(Bhi+Blo)^T / 64 + bias); bn = B tile rows (256 or 64)
+// tensor-core GEMM launch: C = act((Ahi+Alo)(Bhi+Blo)^T / 64 + bias); bn = B tile rows (256 or 64).
+// The BN = 256 instances store through TMA: each output they write needs its store map (sc for c32, sh / sl for
+// oh / ol), built where the buffer is allocated, of [M rows, N columns].
 struct TcOut {
   float* c32 = nullptr; int ldc = 0;
   __half *oh = nullptr, *ol = nullptr; int ldh = 0;
+  const TcStoreMap *sc = nullptr, *sh = nullptr, *sl = nullptr;
 };
 void gemm_tc(cn_policy* p, cudaStream_t st, const TcMat& A, const TcMat& B, int M, int N, int K, int bn, const float* bias,
              int act, const TcOut& o, const int* m_ptr = nullptr, int act_lo = 0, int act_hi = 1 << 30,
@@ -257,16 +302,35 @@ void gemm_tc(cn_policy* p, cudaStream_t st, const TcMat& A, const TcMat& B, int 
 #ifdef CN_GEMM_TRACE
   ep.trace = g_tc_trace; ep.trace_cap = g_tc_trace_cap;
 #endif
+  static const CUtensorMap no_map = {};                 // placeholder for the store maps an instance does not read
+  const CUtensorMap *mc = &no_map, *mh = &no_map, *ml = &no_map;
+  if (bn == 256) {
+    // TMA stores: every output needs a map of exactly [M, N] (the row extent clips the last tile's rows)
+    auto fits = [&](const TcStoreMap* s) { return s && s->rows == M && s->cols == N; };
+    const bool ok = (!o.c32 || fits(o.sc)) && (!o.oh || (fits(o.sh) && fits(o.sl)));
+    if (!ok) {
+      if (!p->launch_error) {
+        p->launch_error = true;
+        cn_set_error("gemm_tc in stage '%s': a BN = 256 output needs a TMA store map of [%d x %d] (16-byte-aligned "
+                     "base, row pitch a multiple of 16 bytes)", p->cur_stage ? p->cur_stage : "?", M, N);
+      }
+      return;
+    }
+    if (o.c32) mc = &o.sc->map;
+    if (o.oh) { mh = &o.sh->map; ml = &o.sl->map; }
+  }
   // persistent: one CTA per SM at most; tiles beyond the device-side row count are never touched
   const int tiles = (N / bn) * ((M + TC_BM - 1) / TC_BM);
   dim3 grid(tiles < p->num_sms ? tiles : p->num_sms);
   if (bn == 256)
-    launch_k(p, tc_kernel<256>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
+    launch_k(p, tc_kernel<256>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep,
+             *mc, *mh, *ml);
   else
-    launch_k(p, tc_kernel<64>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep);
+    launch_k(p, tc_kernel<64>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep,
+             *mc, *mh, *ml);
 }
-TcOut out32(float* c, int ldc) { TcOut o; o.c32 = c; o.ldc = ldc; return o; }
-TcOut out16(const TcMat& t) { TcOut o; o.oh = t.hi; o.ol = t.lo; o.ldh = t.pitch; return o; }
+TcOut out32(float* c, int ldc, const TcStoreMap* sc = nullptr) { TcOut o; o.c32 = c; o.ldc = ldc; o.sc = sc; return o; }
+TcOut out16(const TcMat& t) { TcOut o; o.oh = t.hi; o.ol = t.lo; o.ldh = t.pitch; o.sh = &t.sh; o.sl = &t.sl; return o; }
 TcOut out_both(float* c, int ldc, const TcMat& t) { TcOut o = out16(t); o.c32 = c; o.ldc = ldc; return o; }
 
 int tc_set_attrs() {
@@ -403,6 +467,9 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     if (!rc) rc = tc_alloc(p, p->tAc1, Ni, 512, TC_BM, tc_box_k(64));
     if (!rc) rc = tc_view(p->tA1, p->tAc1, 0, Ni, 256, TC_BM);          // actor.0 half
     if (!rc) rc = tc_view(p->tC1, p->tAc1, 256, Ni, 256, TC_BM);        // critic.0 half
+    // fp32 outputs of the BN = 256 GEMMs (qkv, outproj_spatial)
+    if (!rc) rc = make_store_map(&p->qkv_st, p->qkv, 4, Mi, 1536, 1536);
+    if (!rc) rc = make_store_map(&p->sout_st, p->sout, 4, Mi, 256, 256);
     if (!rc) rc = tc_set_attrs();
   }
   if (rc) { cn_policy_destroy(p); return rc; }
@@ -647,18 +714,18 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
                getenv("CN_QA_DBG") ? atoi(getenv("CN_QA_DBG")) : 0);
       mark(p, st, 4);
     } else if (p->qkv_chunks == 1) {
-      gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536), mc);
+      gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
       mark(p, st, 4);
       launch_k(p, p->attn_kernel, dim3(p->num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
                                                                              nullptr, ah, al);
     } else {
-    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536), mid);
+    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mid);
     cudaEventRecord(p->ev_fork3, st);
     cudaStreamWaitEvent(p->st3, p->ev_fork3, 0);
     launch_k(p, p->attn_kernel, dim3(p->num_sms * 32 / p->attn_warps), dim3(p->attn_warps * 32), 0, p->st3, p->qkv, p->row_start, p->row_env, mid, nullptr,
                                                                               nullptr, ah, al);
     cudaEventRecord(p->ev_join3, p->st3);
-    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536), mc, 0, 1 << 30, mid);
+    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
     mark(p, st, 4);
     launch_k(p, p->attn_kernel, dim3(p->num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
                                                                            ah, al);
@@ -671,7 +738,7 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
                                                                            p->ao, nullptr, nullptr);
   }
   mark(p, st, 5);
-  if (tcm) gemm_tc(p, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256), mc);
+  if (tcm) gemm_tc(p, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
   else gemm(p, st, p->ao, 512, p->Wos, 512, p->bos, p->sout, 256, M, 256, 512, CN_ACT_RELU, 0, ALL, mc);
   // 2. join the robot branch
   mark(p, st, 6);
@@ -746,6 +813,11 @@ int cn_internal_gemm_tc_ex(const float* dA, const float* dW, const float* dbias,
       (out_hi && ldh < N))
     return cn_set_error("cn_internal_gemm_tc_ex: need bn in {64,256}, M, N, K > 0, N %% bn == 0, K %% 64 == 0, "
                         "a_col0 + K <= a_pitch (both multiples of 8), an output and ldh >= N");
+  // the BN = 256 instances store with TMA (gemm_tc); check here, before anything is launched
+  if (bn == 256 && ((dC && !tma_store_ok(dC, (size_t)N * 4)) ||
+                    (out_hi && (!tma_store_ok(out_hi, (size_t)ldh * 2) || !tma_store_ok(out_lo, (size_t)ldh * 2)))))
+    return cn_set_error("cn_internal_gemm_tc_ex: a BN = 256 output needs a 16-byte-aligned base and a row pitch that is "
+                        "a multiple of 16 bytes");
   cn_policy tmp;
   tmp.launches = 0;
   tmp.st2 = nullptr; tmp.st3 = nullptr;
@@ -756,11 +828,18 @@ int cn_internal_gemm_tc_ex(const float* dA, const float* dW, const float* dbias,
   if (!rc) rc = tc_view(A, Af, a_col0, M, K, TC_BM);
   if (!rc) rc = tc_alloc(&tmp, B, N, K, bn, tc_box_k(bn));
   if (!rc) rc = tc_set_attrs();
+  TcOut o = out32(dC, N);
+  o.oh = out_hi; o.ol = out_lo; o.ldh = ldh;
+  TcStoreMap sc, sh, sl;                           // store maps of this call's outputs (BN = 256)
+  if (bn == 256) {
+    if (!rc && dC) rc = make_store_map(&sc, dC, 4, M, N, N);
+    if (!rc && out_hi) rc = make_store_map(&sh, out_hi, 2, M, N, ldh);
+    if (!rc && out_hi) rc = make_store_map(&sl, out_lo, 2, M, N, ldh);
+    o.sc = &sc; o.sh = &sh; o.sl = &sl;
+  }
   if (!rc) {
     split16(&tmp, 0, dA, 1.0f, Af.hi, Af.lo, (size_t)M * a_pitch);
     split16(&tmp, 0, dW, 64.0f, B.hi, B.lo, (size_t)N * K);
-    TcOut o = out32(dC, N);
-    o.oh = out_hi; o.ol = out_lo; o.ldh = ldh;
     gemm_tc(&tmp, 0, A, B, M, N, K, bn, dbias, act, o, m_ptr, act_lo, act_hi > 0 ? act_hi : 1 << 30, m0_ptr);
     cudaError_t err = cudaDeviceSynchronize();
     if (err != cudaSuccess) rc = cn_set_error("cn_internal_gemm_tc_ex: %s", cudaGetErrorString(err));
@@ -777,7 +856,7 @@ int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, fl
 
 #ifdef CN_GEMM_TRACE
 // Traced builds only (tools/gemm_tile_trace.py): every following gemm_tc launch writes per-tile records
-// [gridDim.x][cap][5] (tile start, first full-barrier pass, main-loop end, epilogue end, failed polls) to dtrace.
+// [gridDim.x][cap][TC_TRACE_REC] (cn_gemm_tc.cuh) to dtrace.
 int cn_internal_gemm_trace(unsigned long long* dtrace, int cap) {
   g_tc_trace = dtrace; g_tc_trace_cap = dtrace ? cap : 0;
   return 0;

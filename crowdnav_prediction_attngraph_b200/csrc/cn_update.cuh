@@ -547,7 +547,9 @@ int launch_gemm(int device, cudaStream_t st, const __half* ahi, const __half* al
   ep.c32 = C; ep.ldc = ldc; ep.inv_scale_a = inv_a; ep.inv_scale_b = inv_b; ep.ksplit = ksplit;
   const int tiles = (b_rows / bn) * ((a_rows + TC_BM - 1) / TC_BM) * (ksplit > 1 ? ksplit : 1);
   const int grid = tiles < g_dev[device].sms ? tiles : g_dev[device].sms;
-  cn_gemm_tc_kernel<64, true><<<grid, TC_THREADS, TcCfg<64>::kSmemBytes, st>>>(mah, mal, mbh, mbl, a_rows, b_rows, Kp, ep);
+  static const CUtensorMap no_map = {};        // the PROMOTE instance stores directly; its store maps are not read
+  cn_gemm_tc_kernel<64, true><<<grid, TC_THREADS, TcCfg<64>::kSmemBytes, st>>>(mah, mal, mbh, mbl, a_rows, b_rows, Kp, ep,
+                                                                                no_map, no_map, no_map);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return cn_set_error("cn_update gemm launch (M=%d N=%d K=%d ksplit=%d): %s", a_rows, b_rows, Kd, ksplit, cudaGetErrorString(e));
   return 0;
