@@ -33,6 +33,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "cn_launch.cuh"
+
 #define TC_BM 128
 #define TC_BK 64                                      // k-block of the BN = 64 instances (and the PPO update's maps)
 #define TC_CONSUMER_WARPS 8                           // two consumer warp groups
@@ -69,7 +71,7 @@ struct TcEpilogue {
   const int* m_ptr;      // optional device-side row count (compacted rows); tiles past it exit
   int dbg_nostore;       // diagnostic: run the epilogue arithmetic but skip the global stores
   const int* m0_ptr;     // optional device-side first row: the launch covers rows [*m0_ptr, *m_ptr) (row chunks)
-  // --- PPO update path (cn_update.cuh); all zero / null in the rollout ---
+  // --- PPO update path (cn_update.cu); all zero / null in the rollout ---
   const float* inv_scale_a;   // optional device scalars: the result is also multiplied by *inv_scale_a * *inv_scale_b
   const float* inv_scale_b;   // (dynamic power-of-two operand scales chosen from the tensors' amax)
   int ksplit;                 // > 1 (PROMOTE only): the K range is cut into `ksplit` slices, every slice is its own tile and ADDS its
@@ -688,16 +690,4 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
   if constexpr (kTmaStore) {
     if (sg.leader) tc::bulk_wait_all();
   }
-}
-
-// fp32 -> (hi, lo) fp16 split with an exact power-of-two pre-scale (weights at finalize time,
-// and the generic "split this activation" helper).
-__global__ void cn_split_f16_kernel(const float* __restrict__ src, float scale, __half* __restrict__ hi,
-                                    __half* __restrict__ lo, size_t count) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const float x = fminf(fmaxf(src[i] * scale, -65504.0f), 65504.0f);
-  const __half h = __float2half_rn(x);
-  hi[i] = h;
-  lo[i] = __float2half_rn(x - __half2float(h));
 }

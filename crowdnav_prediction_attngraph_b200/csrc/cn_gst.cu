@@ -13,7 +13,7 @@
 // relative positions written into the 2(P+1)-wide spatial_edges rows, rows sorted by distance to the robot.
 // All activations live in shared memory; weights are stored transposed ([K][N]) so the register-tiled dense
 // layers read them coalesced (they stay L2 resident: 269 KB).  fp32 CUDA cores: this first version favours
-// parity (<= 2e-5 on the predicted positions).  The default path since is cn_gst_tc.cuh (batched wgmma GEMMs over
+// parity (<= 2e-5 on the predicted positions).  The default path since is cn_gst_tc.cu (batched wgmma GEMMs over
 // all environments + row-wise kernels); this fused kernel stays as CN_GST_MODE=fused (one launch, no workspace).
 #include <cuda_runtime.h>
 #include <math.h>
@@ -346,7 +346,7 @@ const int kNumParams = 20;
 
 }  // namespace
 
-// tensor-core implementation (cn_gst_tc.cuh, compiled inside cn_policy.cu)
+// tensor-core implementation (cn_gst_tc.cu)
 void* cn_gst_tc_create(int N, int H, int P, float thr, float pen, int device, const float* const* host, const int* rows,
                        const int* cols);
 void cn_gst_tc_destroy(void* handle);
@@ -456,7 +456,7 @@ int cn_gst_finalize(cn_gst* g) {
     g->allocs.push_back(q);
     g->dev[i] = (const float*)q;
   }
-  // default: dense layers as batched tensor-core GEMMs over all environments (cn_gst_tc.cuh, 2.5x faster at N = 4096);
+  // default: dense layers as batched tensor-core GEMMs over all environments (cn_gst_tc.cu, 2.5x faster at N = 4096);
   // CN_GST_MODE=fused selects the single fused CUDA-core kernel of this file (no workspace, one launch)
   const char* mode = getenv("CN_GST_MODE");
   g->compact = !(mode && strcmp(mode, "tc") == 0);          // default "tcc": compact rows; "tc": every row

@@ -20,36 +20,15 @@
 
 #include "../../include/crowdnav_b200.h"
 #include "cn_host_util.h"
+#include "cn_gemm_tc.h"
+#include "cn_launch.cuh"
 #include "cn_policy_kernels.cuh"
-#include "cn_gemm_tc.cuh"
 #include "cn_qkv_attn.cuh"
-
-// TMA store map of an output of the BN = 256 GEMM instances: [rows, cols], boxes of 64 rows x 128 bytes, 128-byte
-// swizzle (cn_gemm_tc.cuh, tc_epilogue_tma).  rows = 0: no map (TMA needs a 16-byte-aligned base and a row pitch that
-// is a multiple of 16 bytes).
-struct TcStoreMap {
-  CUtensorMap map;
-  int rows = 0, cols = 0;
-};
-
-// A split-fp16 matrix [rows, K] (row pitch `pitch` elements) and its TMA descriptors.
-struct TcMat {
-  __half *hi = nullptr, *lo = nullptr;
-  CUtensorMap mh, ml;
-  int pitch = 0;
-  int box_k = 0;   // k width of the TMA box of mh / ml: the k-block of the GEMM instance that reads it
-  TcStoreMap sh, sl;   // store maps of hi / lo, for a BN = 256 GEMM that writes this matrix
-};
 
 struct cn_policy {
   cn_policy_config cfg;
   int N, H, Win, M;
-  int64_t launches;
-  int num_sms;
-  bool pdl;           // programmatic dependent launch along the kernel chain (CN_PDL=0 disables)
-  long dbg_launch_idx = 0;   // launch index within the current step (CN_PDL_WINDOW debugging)
-  bool launch_error;  // a launch or a GEMM output map failed (cn_last_error has the stage and the reason)
-  const char* cur_stage = nullptr;   // stage name of the launches being enqueued (error reports)
+  CnLaunchCtx lc;     // launch counter, PDL, first launch error, device allocations
   bool fuse_qkv;      // QKV projection + human-human attention in ONE kernel (cn_qkv_attn.cuh; opt-in, CN_FUSE_QKV=1)
   TcMat tWqkvH;       // folded QKV weight, rows head-major: [8][Q 64 | K 64 | V 64][512]
   CUtensorMap qa_ah, qa_al, qa_bh, qa_bl;   // 32-wide (SWIZZLE_64B) boxes of tE2 and tWqkvH for the fused kernel
@@ -63,8 +42,7 @@ struct cn_policy {
   int qkv_chunks;     // 1 (default): single pass; 2 (CN_QKV_CHUNKS=2): QKV + attention in two row chunks with overlap
   bool finalized;
   std::map<std::string, std::vector<float>> host;
-  std::vector<void*> allocs;
-  size_t ws_allocs;   // allocs[0..ws_allocs) = workspace (kept); the rest = parameters of the last finalize
+  size_t ws_allocs;   // lc.allocs[0..ws_allocs) = workspace (kept); the rest = parameters of the last finalize
   // device parameters (fp32 kernel layouts)
   float *W1, *b1, *W2, *b2, *Wqkv, *bqkv, *Wos, *bos;
   float *Wr, *br, *Wet, *bet, *WsT, *bs, *Wa, *ba, *Wih, *bih, *Whh, *bhh, *Wo, *bo;
@@ -90,18 +68,8 @@ struct cn_policy {
 
 namespace {
 
-int palloc(cn_policy* p, float** ptr, size_t count) {
-  void* q = nullptr;
-  cudaError_t err = cudaMalloc(&q, (count ? count : 4) * sizeof(float));
-  if (err != cudaSuccess) return cn_set_error("cudaMalloc(%zu floats): %s", count, cudaGetErrorString(err));
-  cudaMemset(q, 0, (count ? count : 4) * sizeof(float));
-  p->allocs.push_back(q);
-  *ptr = static_cast<float*>(q);
-  return 0;
-}
-
 int upload(cn_policy* p, float** dst, const std::vector<float>& src) {
-  int rc = palloc(p, dst, src.size());
+  int rc = palloc(&p->lc, dst, src.size());
   if (rc) return rc;
   cudaError_t err = cudaMemcpy(*dst, src.data(), src.size() * sizeof(float), cudaMemcpyHostToDevice);
   if (err != cudaSuccess) return cn_set_error("H2D param: %s", cudaGetErrorString(err));
@@ -118,241 +86,11 @@ const std::vector<float>* get(cn_policy* p, const char* key, size_t count) {
   return &it->second;
 }
 
-typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                             const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                             CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeFn get_encode() {
-  static EncodeFn fn = nullptr;
-  if (!fn) {
-    void* sym = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeFn>(sym);
-  }
-  return fn;
-}
-
-// 2-D fp16 row-major [rows, K] tensor with row pitch `pitch`, box = 64 (K) x box_rows, 128-byte swizzle
-// (box_k = 32: 64-byte rows with SWIZZLE_64B, the half-width K blocks of cn_qkv_attn.cuh)
-int make_map(CUtensorMap* map, const __half* ptr, int rows, int K, int box_rows, int pitch, int box_k = TC_BK) {
-  EncodeFn enc = get_encode();
-  if (!enc) return cn_set_error("cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)pitch * sizeof(__half)};
-  cuuint32_t box[2] = {(cuuint32_t)box_k, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, box_k == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return cn_set_error("cuTensorMapEncodeTiled failed (%d) rows=%d K=%d", (int)r, rows, K);
-  return 0;
-}
-
-int halloc16(cn_policy* p, __half** ptr, size_t count) {
-  float* q = nullptr;
-  int rc = palloc(p, &q, (count + 1) / 2);
-  *ptr = reinterpret_cast<__half*>(q);
-  return rc;
-}
-
-// k width of the TMA boxes of the GEMM instance with B-tile rows bn (32 for BN = 256, 64 for BN = 64)
-int tc_box_k(int bn) { return bn == 256 ? TcCfg<256>::kBK : TcCfg<64>::kBK; }
-
-// TMA can store a box into a matrix with this base and row pitch (bytes)
-bool tma_store_ok(const void* ptr, size_t pitch_bytes) { return ((uintptr_t)ptr % 16) == 0 && pitch_bytes % 16 == 0; }
-
-// store map of a BN = 256 output: fp32 (esize 4) or fp16 (esize 2) [rows, cols], row pitch `pitch` elements
-int make_store_map(TcStoreMap* s, const void* ptr, int esize, int rows, int cols, int pitch) {
-  s->rows = s->cols = 0;
-  if (!tma_store_ok(ptr, (size_t)pitch * esize))
-    return cn_set_error("TMA store map: base %p / row pitch %d B not 16-byte aligned", ptr, pitch * esize);
-  EncodeFn enc = get_encode();
-  if (!enc) return cn_set_error("cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)pitch * esize};
-  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), 64};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(&s->map, esize == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                   const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return cn_set_error("cuTensorMapEncodeTiled(store) failed (%d) rows=%d cols=%d", (int)r, rows, cols);
-  s->rows = rows; s->cols = cols;
-  return 0;
-}
-// store maps of the hi / lo halves of a split matrix (left empty where TMA cannot store: an unaligned column view)
-int tc_store_maps(TcMat& t, int rows, int K) {
-  if (!tma_store_ok(t.hi, (size_t)t.pitch * 2) || !tma_store_ok(t.lo, (size_t)t.pitch * 2)) return 0;
-  int rc = make_store_map(&t.sh, t.hi, 2, rows, K, t.pitch);
-  if (!rc) rc = make_store_map(&t.sl, t.lo, 2, rows, K, t.pitch);
-  return rc;
-}
-
-// allocate a split matrix [rows, K] and build its maps (box_rows = 128 for A operands, BN for B operands;
-// box_k = tc_box_k(BN) of the instance that reads it)
-int tc_alloc(cn_policy* p, TcMat& t, int rows, int K, int box_rows, int box_k) {
-  int rc = halloc16(p, &t.hi, (size_t)rows * K);
-  if (!rc) rc = halloc16(p, &t.lo, (size_t)rows * K);
-  t.pitch = K; t.box_k = box_k;
-  if (!rc) rc = make_map(&t.mh, t.hi, rows, K, box_rows, K, box_k);
-  if (!rc) rc = make_map(&t.ml, t.lo, rows, K, box_rows, K, box_k);
-  if (!rc) rc = tc_store_maps(t, rows, K);
-  return rc;
-}
-// view of columns [col0, col0 + K) of an existing split matrix (same box width as the source)
-int tc_view(TcMat& v, const TcMat& src, int col0, int rows, int K, int box_rows) {
-  v.hi = src.hi + col0; v.lo = src.lo + col0; v.pitch = src.pitch; v.box_k = src.box_k;
-  int rc = make_map(&v.mh, v.hi, rows, K, box_rows, src.pitch, src.box_k);
-  if (!rc) rc = make_map(&v.ml, v.lo, rows, K, box_rows, src.pitch, src.box_k);
-  if (!rc) rc = tc_store_maps(v, rows, K);
-  return rc;
-}
-
-// Kernel launch with (optionally) programmatic dependent launch: the kernel may be scheduled before its
-// predecessor in the stream has finished; every kernel of the chain calls griddepcontrol.wait before touching
-// global memory (cn_pdl_prologue / cn_pdl_wait), so the data dependencies are unchanged.
-template <typename... KArgs, typename... Args>
-void launch_k(cn_policy* p, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  // debug aid: CN_PDL_WINDOW=lo:hi keeps the attribute only for launches lo <= index < hi of the context
-  static int win_lo = -1, win_hi = -1;
-  if (win_lo < 0) {
-    const char* w = getenv("CN_PDL_WINDOW");
-    win_lo = 0; win_hi = 1 << 30;
-    if (w) sscanf(w, "%d:%d", &win_lo, &win_hi);
-  }
-  const long idx = p->dbg_launch_idx++;
-  cfg.attrs = at; cfg.numAttrs = (p->pdl && idx >= win_lo && idx < win_hi) ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-  if (e != cudaSuccess && !p->launch_error) {     // keep the FIRST failure and the stage it happened in
-    p->launch_error = true;
-    cn_set_error("kernel launch failed in stage '%s' (launch #%lld of this handle): %s",
-                 p->cur_stage ? p->cur_stage : "?", (long long)p->launches, cudaGetErrorString(e));
-  }
-  p->launches += 1;
-}
-
-void split16(cn_policy* p, cudaStream_t st, const float* src, float scale, __half* hi, __half* lo, size_t count) {
-  cn_split_f16_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(src, scale, hi, lo, count);
-  p->launches += 1;
-}
-
-// the non-PROMOTE instance of cn_gemm_tc_kernel with B-tile rows BN, activation act (CN_ACT_*) and output kind out (TC_OUT_*)
-typedef void (*TcKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, int, int, int, TcEpilogue, CUtensorMap,
-                         CUtensorMap, CUtensorMap);
-template <int BN>
-TcKernel tc_kernel(int act, int out) {
-  static const TcKernel k[3][3] = {
-      {cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_F16>,
-       cn_gemm_tc_kernel<BN, false, CN_ACT_NONE, TC_OUT_BOTH>},
-      {cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_F16>,
-       cn_gemm_tc_kernel<BN, false, CN_ACT_RELU, TC_OUT_BOTH>},
-      {cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_F32>, cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_F16>,
-       cn_gemm_tc_kernel<BN, false, CN_ACT_TANH, TC_OUT_BOTH>}};
-  return k[act][out - 1];
-}
-
-#ifdef CN_GEMM_TRACE
-unsigned long long* g_tc_trace = nullptr;   // per-tile trace buffer of every following gemm_tc launch (or null)
-int g_tc_trace_cap = 0;
-#endif
-
-// tensor-core GEMM launch: C = act((Ahi+Alo)(Bhi+Blo)^T / 64 + bias); bn = B tile rows (256 or 64).
-// The BN = 256 instances store through TMA: each output they write needs its store map (sc for c32, sh / sl for
-// oh / ol), built where the buffer is allocated, of [M rows, N columns].
-struct TcOut {
-  float* c32 = nullptr; int ldc = 0;
-  __half *oh = nullptr, *ol = nullptr; int ldh = 0;
-  const TcStoreMap *sc = nullptr, *sh = nullptr, *sl = nullptr;
-};
-void gemm_tc(cn_policy* p, cudaStream_t st, const TcMat& A, const TcMat& B, int M, int N, int K, int bn, const float* bias,
-             int act, const TcOut& o, const int* m_ptr = nullptr, int act_lo = 0, int act_hi = 1 << 30,
-             const int* m0_ptr = nullptr) {
-  TcEpilogue ep;
-  memset(&ep, 0, sizeof(ep));
-  ep.bias = bias; ep.inv_scale = 1.0f / 64.0f; ep.act = act; ep.act_lo = act_lo; ep.act_hi = act_hi;
-  ep.c32 = o.c32; ep.ldc = o.ldc; ep.out_hi = o.oh; ep.out_lo = o.ol; ep.ldh = o.ldh; ep.m_ptr = m_ptr; ep.m0_ptr = m0_ptr;
-  {
-    static const int nostore = (getenv("CN_DBG_NOSTORE") && getenv("CN_DBG_NOSTORE")[0] == '1') ? 1 : 0;
-    ep.dbg_nostore = nostore;
-  }
-  // the operand maps must have the box width this instance loads, or its barriers would wait for bytes that never come
-  if (A.box_k != tc_box_k(bn) || B.box_k != tc_box_k(bn)) {
-    if (!p->launch_error) {
-      p->launch_error = true;
-      cn_set_error("gemm_tc in stage '%s': operand boxes %d / %d wide, the BN = %d instance loads %d",
-                   p->cur_stage ? p->cur_stage : "?", A.box_k, B.box_k, bn, tc_box_k(bn));
-    }
-    return;
-  }
-  const int out_kind = (o.c32 ? TC_OUT_F32 : 0) | (o.oh ? TC_OUT_F16 : 0);
-  if (act < CN_ACT_NONE || act > CN_ACT_TANH || !out_kind) {
-    if (!p->launch_error) {
-      p->launch_error = true;
-      cn_set_error("gemm_tc in stage '%s': activation %d / no output", p->cur_stage ? p->cur_stage : "?", act);
-    }
-    return;
-  }
-#ifdef CN_GEMM_TRACE
-  ep.trace = g_tc_trace; ep.trace_cap = g_tc_trace_cap;
-#endif
-  static const CUtensorMap no_map = {};                 // placeholder for the store maps an instance does not read
-  const CUtensorMap *mc = &no_map, *mh = &no_map, *ml = &no_map;
-  if (bn == 256) {
-    // TMA stores: every output needs a map of exactly [M, N] (the row extent clips the last tile's rows)
-    auto fits = [&](const TcStoreMap* s) { return s && s->rows == M && s->cols == N; };
-    const bool ok = (!o.c32 || fits(o.sc)) && (!o.oh || (fits(o.sh) && fits(o.sl)));
-    if (!ok) {
-      if (!p->launch_error) {
-        p->launch_error = true;
-        cn_set_error("gemm_tc in stage '%s': a BN = 256 output needs a TMA store map of [%d x %d] (16-byte-aligned "
-                     "base, row pitch a multiple of 16 bytes)", p->cur_stage ? p->cur_stage : "?", M, N);
-      }
-      return;
-    }
-    if (o.c32) mc = &o.sc->map;
-    if (o.oh) { mh = &o.sh->map; ml = &o.sl->map; }
-  }
-  // persistent: one CTA per SM at most; tiles beyond the device-side row count are never touched
-  const int tiles = (N / bn) * ((M + TC_BM - 1) / TC_BM);
-  dim3 grid(tiles < p->num_sms ? tiles : p->num_sms);
-  if (bn == 256)
-    launch_k(p, tc_kernel<256>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep,
-             *mc, *mh, *ml);
-  else
-    launch_k(p, tc_kernel<64>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep,
-             *mc, *mh, *ml);
-}
-TcOut out32(float* c, int ldc, const TcStoreMap* sc = nullptr) { TcOut o; o.c32 = c; o.ldc = ldc; o.sc = sc; return o; }
-TcOut out16(const TcMat& t) { TcOut o; o.oh = t.hi; o.ol = t.lo; o.ldh = t.pitch; o.sh = &t.sh; o.sl = &t.sl; return o; }
-TcOut out_both(float* c, int ldc, const TcMat& t) { TcOut o = out16(t); o.c32 = c; o.ldc = ldc; return o; }
-
-int tc_set_attrs() {
-  cudaError_t e = cudaSuccess;
-  for (int act = CN_ACT_NONE; act <= CN_ACT_TANH; ++act)
-    for (int out = TC_OUT_F32; out <= TC_OUT_BOTH; ++out) {
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(tc_kernel<256>(act, out), cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<256>::kSmemBytes);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(tc_kernel<64>(act, out), cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::kSmemBytes);
-    }
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(cn_qkv_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QA_SMEM_BYTES);
-  if (e != cudaSuccess) return cn_set_error("cudaFuncSetAttribute(tc): %s", cudaGetErrorString(e));
-  return 0;
-}
-
 void gemm(cn_policy* p, cudaStream_t st, const float* A, int lda, const float* W, int ldw, const float* bias,
           float* C, int ldc, int M, int N, int K, int act, int act_lo = 0, int act_hi = 1 << 30,
           const int* m_ptr = nullptr, __half* oh = nullptr, __half* ol = nullptr) {
   dim3 grid((N + CN_GEMM_BN - 1) / CN_GEMM_BN, (M + CN_GEMM_BM - 1) / CN_GEMM_BM);
-  launch_k(p, cn_gemm_f32_kernel, grid, dim3(256), 0, st, A, lda, W, ldw, bias, C, ldc, M, N, K, act, act_lo, act_hi, m_ptr, oh, ol);
+  launch_k(&p->lc, cn_gemm_f32_kernel, grid, dim3(256), 0, st, A, lda, W, ldw, bias, C, ldc, M, N, K, act, act_lo, act_hi, m_ptr, oh, ol);
 }
 
 const char* kStageNames[] = {"pack_inputs", "embed1_gemm", "embed2_gemm", "qkv_gemm", "hh_attention",
@@ -360,7 +98,7 @@ const char* kStageNames[] = {"pack_inputs", "embed1_gemm", "embed2_gemm", "qkv_g
 const int kNumStages = sizeof(kStageNames) / sizeof(kStageNames[0]);
 
 inline void mark(cn_policy* p, cudaStream_t st, int i) {
-  p->cur_stage = i < kNumStages ? kStageNames[i] : "end";
+  p->lc.cur_stage = i < kNumStages ? kStageNames[i] : "end";
   if (p->profile) cudaEventRecord(p->ev[i], st);
 }
 
@@ -406,12 +144,9 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
   cn_policy* p = new cn_policy();
   p->cfg = *cfg;
   p->N = cfg->num_envs; p->H = cfg->human_num; p->Win = cfg->input_size; p->M = p->N * p->H;
-  p->launches = 0; p->finalized = false; p->profile = false; p->launch_error = false;
-  p->num_sms = 132;
-  cudaDeviceGetAttribute(&p->num_sms, cudaDevAttrMultiProcessorCount, cfg->device);
+  p->finalized = false; p->profile = false;
+  cn_launch_init(&p->lc, cfg->device);
   {
-    const char* pd = getenv("CN_PDL");
-    p->pdl = !(pd && pd[0] == '0');
     const char* qc = getenv("CN_QKV_CHUNKS");
     p->qkv_chunks = (qc && qc[0] == '2') ? 2 : 1;
     const char* ar = getenv("CN_ATTN_R");
@@ -435,16 +170,16 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
   const size_t M = (size_t)p->M, N = (size_t)p->N;
   const int Mi = p->M, Ni = p->N;
   int rc = 0;
-#define WS(name, count) if (!rc) rc = palloc(p, &p->name, (count))
+#define WS(name, count) if (!rc) rc = palloc(&p->lc, &p->name, (count))
   {
     float* q = nullptr;
-    if (!rc) rc = palloc(p, &q, N + 2);
+    if (!rc) rc = palloc(&p->lc, &q, N + 2);
     p->row_start = reinterpret_cast<int*>(q);
-    if (!rc) rc = palloc(p, &q, 4);
+    if (!rc) rc = palloc(&p->lc, &q, 4);
     p->mc = reinterpret_cast<int*>(q);
-    if (!rc) rc = palloc(p, &q, M + 1);
+    if (!rc) rc = palloc(&p->lc, &q, M + 1);
     p->row_env = reinterpret_cast<int*>(q);
-    if (!rc) rc = palloc(p, &q, 2 * N + 4);
+    if (!rc) rc = palloc(&p->lc, &q, 2 * N + 4);
     p->tile_tab = reinterpret_cast<int*>(q);
   }
   WS(x16, M * 16); WS(e1, M * 128); WS(e2, M * 512); WS(qkv, M * 1536); WS(ao, M * 512); WS(sout, M * 256);
@@ -454,26 +189,30 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
   if (!rc && cfg->gemm_mode == 1) {
     // A operands: box rows = 128 (TC_BM)
     // per-human rows feed the BN = 256 instance, per-environment rows the BN = 64 one
-    rc = tc_alloc(p, p->tE1, Mi, 128, TC_BM, tc_box_k(256));
-    if (!rc) rc = tc_alloc(p, p->tE2, Mi, 512, TC_BM, tc_box_k(256));
-    if (!rc) rc = tc_alloc(p, p->tAo, Mi, 512, TC_BM, tc_box_k(256));
-    if (!rc) rc = tc_alloc(p, p->tRs, Ni, 256, TC_BM, tc_box_k(64));
-    if (!rc) rc = tc_alloc(p, p->tT1, Ni, 128, TC_BM, tc_box_k(64));   // [enc | te] then [enc | emb]
+    rc = tc_alloc(&p->lc, p->tE1, Mi, 128, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(&p->lc, p->tE2, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(&p->lc, p->tAo, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc) rc = tc_alloc(&p->lc, p->tRs, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tT1, Ni, 128, TC_BM, tc_box_k(64));   // [enc | te] then [enc | emb]
     if (!rc) rc = tc_view(p->tTe, p->tT1, 64, Ni, 64, TC_BM);           // te = columns 64..127
-    if (!rc) rc = tc_alloc(p, p->tWv, Ni, 256, TC_BM, tc_box_k(64));
-    if (!rc) rc = tc_alloc(p, p->tH0, Ni, 128, TC_BM, tc_box_k(64));
-    if (!rc) rc = tc_alloc(p, p->tH1, Ni, 128, TC_BM, tc_box_k(64));
-    if (!rc) rc = tc_alloc(p, p->tOut, Ni, 256, TC_BM, tc_box_k(64));
-    if (!rc) rc = tc_alloc(p, p->tAc1, Ni, 512, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tWv, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tH0, Ni, 128, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tH1, Ni, 128, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tOut, Ni, 256, TC_BM, tc_box_k(64));
+    if (!rc) rc = tc_alloc(&p->lc, p->tAc1, Ni, 512, TC_BM, tc_box_k(64));
     if (!rc) rc = tc_view(p->tA1, p->tAc1, 0, Ni, 256, TC_BM);          // actor.0 half
     if (!rc) rc = tc_view(p->tC1, p->tAc1, 256, Ni, 256, TC_BM);        // critic.0 half
     // fp32 outputs of the BN = 256 GEMMs (qkv, outproj_spatial)
     if (!rc) rc = make_store_map(&p->qkv_st, p->qkv, 4, Mi, 1536, 1536);
     if (!rc) rc = make_store_map(&p->sout_st, p->sout, 4, Mi, 256, 256);
     if (!rc) rc = tc_set_attrs();
+    if (!rc) {
+      err = cudaFuncSetAttribute(cn_qkv_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QA_SMEM_BYTES);
+      if (err != cudaSuccess) rc = cn_set_error("cudaFuncSetAttribute(qkv_attn): %s", cudaGetErrorString(err));
+    }
   }
   if (rc) { cn_policy_destroy(p); return rc; }
-  p->ws_allocs = p->allocs.size();
+  p->ws_allocs = p->lc.allocs.size();
   *out = p;
   return 0;
 }
@@ -481,7 +220,7 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
 int cn_policy_destroy(cn_policy* p) {
   if (!p) return 0;
   cudaSetDevice(p->cfg.device);
-  for (void* q : p->allocs) cudaFree(q);
+  cn_launch_free(&p->lc);
   for (auto& e : p->ev) cudaEventDestroy(e);
   if (p->st2) {
     cudaStreamDestroy(p->st2);
@@ -553,8 +292,8 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
 #undef GET
   // release device parameters of a previous finalize (workspace allocations come first and stay)
   cudaStreamSynchronize(st);
-  for (size_t i = p->ws_allocs; i < p->allocs.size(); ++i) cudaFree(p->allocs[i]);
-  p->allocs.resize(p->ws_allocs);
+  for (size_t i = p->ws_allocs; i < p->lc.allocs.size(); ++i) cudaFree(p->lc.allocs[i]);
+  p->lc.allocs.resize(p->ws_allocs);
   int rc = 0;
   auto pad_k = [](const std::vector<float>& w, int rows, int k, int kp) {
     std::vector<float> o((size_t)rows * kp, 0.0f);
@@ -591,12 +330,12 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
   if (!rc) rc = upload(p, &d_bout, *bout);
   if (!rc) rc = upload(p, &d_wsl, *wsl);
   if (!rc) rc = upload(p, &d_bsl, *bsl);
-  if (!rc) rc = palloc(p, &p->Wqkv, (size_t)1536 * 512);
-  if (!rc) rc = palloc(p, &p->bqkv, 1536);
-  if (!rc) rc = palloc(p, &p->Wos, (size_t)256 * 512);
-  if (!rc) rc = palloc(p, &p->bos, 256);
-  if (!rc) rc = palloc(p, &p->Woac, (size_t)512 * 128);
-  if (!rc) rc = palloc(p, &p->boac, 512);
+  if (!rc) rc = palloc(&p->lc, &p->Wqkv, (size_t)1536 * 512);
+  if (!rc) rc = palloc(&p->lc, &p->bqkv, 1536);
+  if (!rc) rc = palloc(&p->lc, &p->Wos, (size_t)256 * 512);
+  if (!rc) rc = palloc(&p->lc, &p->bos, 256);
+  if (!rc) rc = palloc(&p->lc, &p->Woac, (size_t)512 * 128);
+  if (!rc) rc = palloc(&p->lc, &p->boac, 512);
   if (rc) return rc;
   for (int i = 0; i < 3; ++i) {
     // Wf_i = Win_i (512x512) @ Wl_i (512x512);  bf_i = Win_i @ bl_i + bin_i
@@ -621,23 +360,23 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
         {p->Wih, &p->tWih, 384, 128, 64},   {p->Whh, &p->tWhh, 384, 128, 64},     {p->Wo, &p->tWo, 256, 128, 64},
         {p->Wac1, &p->tWac1, 512, 256, 64}, {p->Wa2, &p->tWa2, 256, 256, 64},     {p->Wc2, &p->tWc2, 256, 256, 64}};
     for (auto& t : tw) {
-      rc = tc_alloc(p, *t.t, t.rows, t.k, t.bn, tc_box_k(t.bn));
+      rc = tc_alloc(&p->lc, *t.t, t.rows, t.k, t.bn, tc_box_k(t.bn));
       if (rc) return rc;
-      split16(p, st, t.src, 64.0f, t.t->hi, t.t->lo, (size_t)t.rows * t.k);
+      split16(&p->lc, st, t.src, 64.0f, t.t->hi, t.t->lo, (size_t)t.rows * t.k);
     }
     if (p->fuse_qkv) {
       // head-major copy of the folded QKV projection for the fused kernel: row h * 192 + s * 64 + d <- row s * 512 + h * 64 + d
       float* wh = nullptr;
-      rc = palloc(p, &wh, (size_t)1536 * 512);
-      if (!rc) rc = palloc(p, &p->bqkvH, 1536);
-      if (!rc) rc = tc_alloc(p, p->tWqkvH, 1536, 512, QA_BN, QA_BK);
+      rc = palloc(&p->lc, &wh, (size_t)1536 * 512);
+      if (!rc) rc = palloc(&p->lc, &p->bqkvH, 1536);
+      if (!rc) rc = tc_alloc(&p->lc, p->tWqkvH, 1536, 512, QA_BN, QA_BK);
       if (!rc) rc = make_map(&p->qa_bh, p->tWqkvH.hi, 1536, 512, QA_BN, 512, QA_BK);
       if (!rc) rc = make_map(&p->qa_bl, p->tWqkvH.lo, 1536, 512, QA_BN, 512, QA_BK);
       if (!rc) rc = make_map(&p->qa_ah, p->tE2.hi, p->M, 512, TC_BM, 512, QA_BK);
       if (!rc) rc = make_map(&p->qa_al, p->tE2.lo, p->M, 512, TC_BM, 512, QA_BK);
       if (rc) return rc;
       cn_head_major_kernel<<<1536, 128, 0, st>>>(p->Wqkv, p->bqkv, wh, p->bqkvH);
-      split16(p, st, wh, 64.0f, p->tWqkvH.hi, p->tWqkvH.lo, (size_t)1536 * 512);
+      split16(&p->lc, st, wh, 64.0f, p->tWqkvH.hi, p->tWqkvH.lo, (size_t)1536 * 512);
     }
   }
   cudaError_t err = cudaStreamSynchronize(st);
@@ -661,9 +400,9 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   mark(p, st, 0);
   // 0. compaction offsets, pack / pad inputs, h0 = h * mask
   {
-    launch_k(p, cn_row_offsets_kernel, dim3(1), dim3(1024), 0, st, d->detected_human_num, N, H, p->row_start, p->mc);
+    launch_k(&p->lc, cn_row_offsets_kernel, dim3(1), dim3(1024), 0, st, d->detected_human_num, N, H, p->row_start, p->mc);
     const int total = (!tcm && M * 16 > N * 128) ? M * 16 : N * 128;
-    launch_k(p, cn_pack_inputs_kernel, dim3((total + 255) / 256), dim3(256), 0, st, d->spatial_edges, p->Win, H, N, p->row_start, p->row_env,
+    launch_k(&p->lc, cn_pack_inputs_kernel, dim3((total + 255) / 256), dim3(256), 0, st, d->spatial_edges, p->Win, H, N, p->row_start, p->row_env,
                                                                tcm ? nullptr : p->x16,
                                                                d->temporal_edges, d->robot_node, d->h_in, d->masks, p->xr,
                                                                p->h0, tcm ? p->tH0.hi : nullptr, tcm ? p->tH0.lo : nullptr);
@@ -674,14 +413,14 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   cudaStreamWaitEvent(s2, p->ev_fork, 0);
   if (p->fuse_qkv) {
     cn_qkv_tiles_kernel<<<1, 1024, 0, s2>>>(p->row_start, N, p->tile_tab);
-    p->launches += 1;
+    p->lc.launches += 1;
     cudaEventRecord(p->ev_tiles, s2);
   }
   if (tcm) {
     gemm(p, s2, p->xr, 16, p->Wr, 16, p->br, nullptr, 256, N, 256, 16, CN_ACT_RELU, 0, ALL, nullptr, p->tRs.hi, p->tRs.lo);
-    gemm_tc(p, s2, p->tRs, p->tWet, N, 128, 256, 64, p->bet, CN_ACT_RELU, out_both(p->t1, 128, p->tT1), nullptr, 0, 64);
-    gemm_tc(p, s2, p->tTe, p->tWsT, N, 256, 64, 64, nullptr, CN_ACT_NONE, out32(p->u, 256));
-    gemm_tc(p, s2, p->tH0, p->tWhh, N, 384, 128, 64, p->bhh, CN_ACT_NONE, out32(p->gh, 384));
+    gemm_tc(&p->lc, s2, p->tRs, p->tWet, N, 128, 256, 64, p->bet, CN_ACT_RELU, out_both(p->t1, 128, p->tT1), nullptr, 0, 64);
+    gemm_tc(&p->lc, s2, p->tTe, p->tWsT, N, 256, 64, 64, nullptr, CN_ACT_NONE, out32(p->u, 256));
+    gemm_tc(&p->lc, s2, p->tH0, p->tWhh, N, 384, 128, 64, p->bhh, CN_ACT_NONE, out32(p->gh, 384));
   } else {
     gemm(p, s2, p->xr, 16, p->Wr, 16, p->br, p->rs, 256, N, 256, 16, CN_ACT_RELU);
     gemm(p, s2, p->rs, 256, p->Wet, 256, p->bet, p->t1, 128, N, 128, 256, CN_ACT_RELU, 0, 64);   // [enc | te]
@@ -692,11 +431,11 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   // 1. human-human branch over the Mc = sum_e n_e valid rows (device-side count p->mc)
   mark(p, st, 1);
   if (tcm) {
-    launch_k(p, cn_embed1_kernel, dim3(p->num_sms * 6), dim3(256), 0, st, d->spatial_edges, p->Win, H, p->row_start, p->row_env, p->mc, p->W1, p->b1,
+    launch_k(&p->lc, cn_embed1_kernel, dim3(p->lc.num_sms * 6), dim3(256), 0, st, d->spatial_edges, p->Win, H, p->row_start, p->row_env, p->mc, p->W1, p->b1,
                                                      p->tE1.hi, p->tE1.lo);
   } else gemm(p, st, p->x16, 16, p->W1, 16, p->b1, p->e1, 128, M, 128, 16, CN_ACT_RELU, 0, ALL, mc);
   mark(p, st, 2);
-  if (tcm) gemm_tc(p, st, p->tE1, p->tW2, M, 512, 128, 256, p->b2, CN_ACT_RELU, out16(p->tE2), mc);
+  if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 512, 128, 256, p->b2, CN_ACT_RELU, out16(p->tE2), mc);
   else gemm(p, st, p->e1, 128, p->W2, 128, p->b2, p->e2, 512, M, 512, 128, CN_ACT_RELU, 0, ALL, mc);
   mark(p, st, 3);
   if (tcm) {
@@ -709,64 +448,64 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
     if (p->fuse_qkv) {
       // one kernel: projection tile (128 rows of whole environments x one head's Q | K | V) -> attention -> tAo
       cudaStreamWaitEvent(st, p->ev_tiles, 0);                 // tile table from the side stream
-      launch_k(p, cn_qkv_attn_kernel, dim3(p->num_sms), dim3(QA_THREADS), QA_SMEM_BYTES, st, p->qa_ah, p->qa_al, p->qa_bh,
+      launch_k(&p->lc, cn_qkv_attn_kernel, dim3(p->lc.num_sms), dim3(QA_THREADS), QA_SMEM_BYTES, st, p->qa_ah, p->qa_al, p->qa_bh,
                p->qa_bl, p->bqkvH, 1.0f / 64.0f, p->tile_tab, p->row_start, p->row_env, ah, al,
                getenv("CN_QA_DBG") ? atoi(getenv("CN_QA_DBG")) : 0);
       mark(p, st, 4);
     } else if (p->qkv_chunks == 1) {
-      gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
+      gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
       mark(p, st, 4);
-      launch_k(p, p->attn_kernel, dim3(p->num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
+      launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
                                                                              nullptr, ah, al);
     } else {
-    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mid);
+    gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mid);
     cudaEventRecord(p->ev_fork3, st);
     cudaStreamWaitEvent(p->st3, p->ev_fork3, 0);
-    launch_k(p, p->attn_kernel, dim3(p->num_sms * 32 / p->attn_warps), dim3(p->attn_warps * 32), 0, p->st3, p->qkv, p->row_start, p->row_env, mid, nullptr,
+    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 32 / p->attn_warps), dim3(p->attn_warps * 32), 0, p->st3, p->qkv, p->row_start, p->row_env, mid, nullptr,
                                                                               nullptr, ah, al);
     cudaEventRecord(p->ev_join3, p->st3);
-    gemm_tc(p, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
+    gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
     mark(p, st, 4);
-    launch_k(p, p->attn_kernel, dim3(p->num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
+    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
                                                                            ah, al);
     cudaStreamWaitEvent(st, p->ev_join3, 0);
     }
   } else {
     gemm(p, st, p->e2, 512, p->Wqkv, 512, p->bqkv, p->qkv, 1536, M, 1536, 512, CN_ACT_NONE, 0, ALL, mc);
     mark(p, st, 4);
-    launch_k(p, p->attn_kernel, dim3(p->num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, p->mc, nullptr,
+    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, p->mc, nullptr,
                                                                            p->ao, nullptr, nullptr);
   }
   mark(p, st, 5);
-  if (tcm) gemm_tc(p, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
+  if (tcm) gemm_tc(&p->lc, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
   else gemm(p, st, p->ao, 512, p->Wos, 512, p->bos, p->sout, 256, M, 256, 512, CN_ACT_RELU, 0, ALL, mc);
   // 2. join the robot branch
   mark(p, st, 6);
   cudaStreamWaitEvent(st, p->ev_join, 0);
   mark(p, st, 7);
-  launch_k(p, cn_hr_attention_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->sout, p->u, p->t1, 128, 64, p->bs, p->row_start, N, H, p->wv,
+  launch_k(&p->lc, cn_hr_attention_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->sout, p->u, p->t1, 128, 64, p->bs, p->row_start, N, H, p->wv,
                                                       tcm ? p->tWv.hi : nullptr, tcm ? p->tWv.lo : nullptr);
   // 3. GRU: emb overwrites the te half of t1 -> t1 = [enc | emb] = GRU input (gh came from the side stream)
   mark(p, st, 8);
   if (tcm) {
     TcOut o; o.oh = p->tT1.hi + 64; o.ol = p->tT1.lo + 64; o.ldh = 128;
-    gemm_tc(p, st, p->tWv, p->tWa, N, 64, 256, 64, p->ba, CN_ACT_RELU, o);
-    gemm_tc(p, st, p->tT1, p->tWih, N, 384, 128, 64, p->bih, CN_ACT_NONE, out32(p->gi, 384));
+    gemm_tc(&p->lc, st, p->tWv, p->tWa, N, 64, 256, 64, p->ba, CN_ACT_RELU, o);
+    gemm_tc(&p->lc, st, p->tT1, p->tWih, N, 384, 128, 64, p->bih, CN_ACT_NONE, out32(p->gi, 384));
   } else {
     gemm(p, st, p->wv, 256, p->Wa, 256, p->ba, p->t1 + 64, 128, N, 64, 256, CN_ACT_RELU);
     gemm(p, st, p->t1, 128, p->Wih, 128, p->bih, p->gi, 384, N, 384, 128, CN_ACT_NONE);
   }
-  launch_k(p, cn_gru_gate_kernel, dim3((N * 128 + 255) / 256), dim3(256), 0, st, p->gi, p->gh, p->h0, N, d->h_out, tcm ? p->tH1.hi : nullptr,
+  launch_k(&p->lc, cn_gru_gate_kernel, dim3((N * 128 + 255) / 256), dim3(256), 0, st, p->gi, p->gh, p->h0, N, d->h_out, tcm ? p->tH1.hi : nullptr,
                                                             tcm ? p->tH1.lo : nullptr);
   // 4. output_linear, actor / critic MLPs (critic.2 on the side stream), heads
   mark(p, st, 9);
   if (tcm) {
-    gemm_tc(p, st, p->tH1, p->tWoac, N, 512, 128, 64, p->boac, CN_ACT_TANH, out16(p->tAc1));     // [actor.0 | critic.0]
+    gemm_tc(&p->lc, st, p->tH1, p->tWoac, N, 512, 128, 64, p->boac, CN_ACT_TANH, out16(p->tAc1));     // [actor.0 | critic.0]
     cudaEventRecord(p->ev_fork2, st);
     cudaStreamWaitEvent(s2, p->ev_fork2, 0);
-    gemm_tc(p, s2, p->tC1, p->tWc2, N, 256, 256, 64, p->bc2, CN_ACT_TANH, out32(p->c2, 256));
+    gemm_tc(&p->lc, s2, p->tC1, p->tWc2, N, 256, 256, 64, p->bc2, CN_ACT_TANH, out32(p->c2, 256));
     cudaEventRecord(p->ev_join2, s2);
-    gemm_tc(p, st, p->tA1, p->tWa2, N, 256, 256, 64, p->ba2, CN_ACT_TANH, out32(p->a2, 256));
+    gemm_tc(&p->lc, st, p->tA1, p->tWa2, N, 256, 256, 64, p->ba2, CN_ACT_TANH, out32(p->a2, 256));
   } else {
     gemm(p, st, d->h_out, 128, p->Woac, 128, p->boac, p->ac1, 512, N, 512, 128, CN_ACT_TANH);
     cudaEventRecord(p->ev_fork2, st);
@@ -776,16 +515,16 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
     gemm(p, st, p->ac1, 512, p->Wa2, 256, p->ba2, p->a2, 256, N, 256, 256, CN_ACT_TANH);
   }
   cudaStreamWaitEvent(st, p->ev_join2, 0);
-  launch_k(p, cn_heads_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->a2, 256, p->c2, 256, p->wv_, p->bv, p->Wm, p->bm, p->logstd, d->noise, N,
+  launch_k(&p->lc, cn_heads_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->a2, 256, p->c2, 256, p->wv_, p->bv, p->Wm, p->bm, p->logstd, d->noise, N,
                                                d->value, d->action, d->log_prob, d->action_mean);
   mark(p, st, kNumStages);
   cudaError_t err = cudaGetLastError();
-  if (p->launch_error) { p->launch_error = false; return 1; }      // cn_last_error names the stage
+  if (p->lc.launch_error) { p->lc.launch_error = false; return 1; }      // cn_last_error names the stage
   if (err != cudaSuccess) return cn_set_error("cn_policy_act launch: %s", cudaGetErrorString(err));
   return 0;
 }
 
-int64_t cn_policy_launch_count(cn_policy* p) { return p ? p->launches : 0; }
+int64_t cn_policy_launch_count(cn_policy* p) { return p ? p->lc.launches : 0; }
 
 int64_t cn_policy_last_rows(cn_policy* p) {
   if (!p) return -1;
@@ -795,73 +534,6 @@ int64_t cn_policy_last_rows(cn_policy* p) {
     return -1;
   return v;
 }
-
-// Internal test hooks (not part of the public header): C = act(A[M,K] W[N,K]^T + bias) through the
-// wgmma 3xFP16 kernel with B-tile rows `bn` (256 or 64), fp32 device pointers in/out.  cn_internal_gemm_tc_ex adds
-// the epilogue and operand variants the rollout uses (zero / null = off):
-//   m_ptr, m0_ptr   device-side row count and first row (rows [*m0_ptr, *m_ptr) of the M-row extent);
-//   a_col0, a_pitch A is the column view [a_col0, a_col0 + K) of an fp32 matrix [M, a_pitch] (pitch 0 = K);
-//   out_hi, out_lo  fp16 (hi, lo) split output with leading dimension ldh (pointers already at the column offset);
-//                   dC may then be null;
-//   act_lo, act_hi  the activation applies to columns [act_lo, act_hi) only (act_hi 0 = all columns).
-int cn_internal_gemm_tc_ex(const float* dA, const float* dW, const float* dbias, float* dC, int M, int N, int K, int act,
-                           int bn, const int* m_ptr, const int* m0_ptr, int a_col0, int a_pitch, __half* out_hi,
-                           __half* out_lo, int ldh, int act_lo, int act_hi) {
-  if (a_pitch == 0) a_pitch = K;
-  if ((bn != 256 && bn != 64) || M <= 0 || N <= 0 || K <= 0 || N % bn || K % TC_BK || a_col0 < 0 ||
-      a_col0 + K > a_pitch || a_col0 % 8 || a_pitch % 8 || (!dC && !out_hi) || (!out_hi != !out_lo) ||
-      (out_hi && ldh < N))
-    return cn_set_error("cn_internal_gemm_tc_ex: need bn in {64,256}, M, N, K > 0, N %% bn == 0, K %% 64 == 0, "
-                        "a_col0 + K <= a_pitch (both multiples of 8), an output and ldh >= N");
-  // the BN = 256 instances store with TMA (gemm_tc); check here, before anything is launched
-  if (bn == 256 && ((dC && !tma_store_ok(dC, (size_t)N * 4)) ||
-                    (out_hi && (!tma_store_ok(out_hi, (size_t)ldh * 2) || !tma_store_ok(out_lo, (size_t)ldh * 2)))))
-    return cn_set_error("cn_internal_gemm_tc_ex: a BN = 256 output needs a 16-byte-aligned base and a row pitch that is "
-                        "a multiple of 16 bytes");
-  cn_policy tmp;
-  tmp.launches = 0;
-  tmp.st2 = nullptr; tmp.st3 = nullptr;
-  tmp.num_sms = 132; tmp.qkv_chunks = 1; tmp.launch_error = false; tmp.pdl = false;
-  cudaDeviceGetAttribute(&tmp.num_sms, cudaDevAttrMultiProcessorCount, 0);
-  TcMat Af, A, B;
-  int rc = tc_alloc(&tmp, Af, M, a_pitch, TC_BM, tc_box_k(bn));
-  if (!rc) rc = tc_view(A, Af, a_col0, M, K, TC_BM);
-  if (!rc) rc = tc_alloc(&tmp, B, N, K, bn, tc_box_k(bn));
-  if (!rc) rc = tc_set_attrs();
-  TcOut o = out32(dC, N);
-  o.oh = out_hi; o.ol = out_lo; o.ldh = ldh;
-  TcStoreMap sc, sh, sl;                           // store maps of this call's outputs (BN = 256)
-  if (bn == 256) {
-    if (!rc && dC) rc = make_store_map(&sc, dC, 4, M, N, N);
-    if (!rc && out_hi) rc = make_store_map(&sh, out_hi, 2, M, N, ldh);
-    if (!rc && out_hi) rc = make_store_map(&sl, out_lo, 2, M, N, ldh);
-    o.sc = &sc; o.sh = &sh; o.sl = &sl;
-  }
-  if (!rc) {
-    split16(&tmp, 0, dA, 1.0f, Af.hi, Af.lo, (size_t)M * a_pitch);
-    split16(&tmp, 0, dW, 64.0f, B.hi, B.lo, (size_t)N * K);
-    gemm_tc(&tmp, 0, A, B, M, N, K, bn, dbias, act, o, m_ptr, act_lo, act_hi > 0 ? act_hi : 1 << 30, m0_ptr);
-    cudaError_t err = cudaDeviceSynchronize();
-    if (err != cudaSuccess) rc = cn_set_error("cn_internal_gemm_tc_ex: %s", cudaGetErrorString(err));
-    else if (tmp.launch_error) rc = 1;
-  }
-  for (void* q : tmp.allocs) cudaFree(q);
-  return rc;
-}
-// the plain form: whole rows, A with pitch K, fp32 output [M, N], activation on every column
-int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, float* dC, int M, int N, int K, int act,
-                        int bn) {
-  return cn_internal_gemm_tc_ex(dA, dW, dbias, dC, M, N, K, act, bn, nullptr, nullptr, 0, 0, nullptr, nullptr, 0, 0, 0);
-}
-
-#ifdef CN_GEMM_TRACE
-// Traced builds only (tools/gemm_tile_trace.py): every following gemm_tc launch writes per-tile records
-// [gridDim.x][cap][TC_TRACE_REC] (cn_gemm_tc.cuh) to dtrace.
-int cn_internal_gemm_trace(unsigned long long* dtrace, int cap) {
-  g_tc_trace = dtrace; g_tc_trace_cap = dtrace ? cap : 0;
-  return 0;
-}
-#endif
 
 // Internal test hook (not part of the public header): where one named workspace buffer of the policy forward lives,
 // so a test can read every stage's input and output back after cn_policy_act.  *kind = 0: fp32 at *ptr; 1: fp16
@@ -928,6 +600,3 @@ int cn_internal_policy_buffer(cn_policy* p, const char* name, void** ptr, void**
 }
 
 }  // extern "C"
-
-#include "cn_gst_tc.cuh"
-#include "cn_update.cuh"

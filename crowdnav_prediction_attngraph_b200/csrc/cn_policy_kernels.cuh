@@ -9,29 +9,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-enum { CN_ACT_NONE = 0, CN_ACT_RELU = 1, CN_ACT_TANH = 2 };
+#include "cn_launch.cuh"
 
 // ------------------------------------------------------------------------------------------
 // fp32 CUDA-core GEMM:  C[M,N] = act(A[M,K] * W[N,K]^T + bias[N]),  act on columns [act_lo, act_hi).
 // 128x128x16 tiles, 256 threads, 8x8 register tile per thread, register-prefetched double
 // buffering through shared memory.  K % 16 == 0 (buffers are zero padded), M and N ragged.
-// Programmatic dependent launch (PDL): kernels of the policy chain are launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization; each one lets its successor be scheduled as early as
-// possible (launch_dependents) and itself waits for the full completion + memory flush of its predecessor
-// (wait) before it touches global memory.  Both are no-ops for a normal launch.
-__device__ __forceinline__ void cn_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void cn_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void cn_pdl_prologue() { cn_pdl_trigger(); cn_pdl_wait(); }
-// Device-side counts written by an earlier kernel of the chain: a plain load through a `const __restrict__` pointer is an
-// invariant load to the compiler, which schedules it ABOVE griddepcontrol.wait (seen in SASS: LDG.CONSTANT before
-// ACQBULK) and so reads the previous step's value.  A volatile asm load stays behind the wait.
-// tools/check_pdl_sass.py (tests/test_build_checks.py) scans the built library for this pattern.
-__device__ __forceinline__ int cn_ld_after_wait(const int* p) {
-  int v;
-  asm volatile("ld.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-
 #define CN_GEMM_BM 128
 #define CN_GEMM_BN 128
 #define CN_GEMM_BK 16

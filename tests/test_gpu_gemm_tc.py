@@ -1,7 +1,8 @@
 """GPU test of the wgmma / TMA GEMM (3xFP16 error-compensated) against an fp64 matmul, through the internal hooks
 cn_internal_gemm_tc and cn_internal_gemm_tc_ex (the epilogue and operand variants the rollout uses: device-side row
 range, column-view A operands, split fp16 outputs at a column offset, activation windows), and of the whole policy
-forward in gemm_mode=1.
+forward in gemm_mode=1.  _check_epilogue_instance is the shared check of the per-instance epilogue tests
+(test_gpu_gemm_tc_epilogue_kinds.py, test_gpu_gemm_tc_tma_store.py).
 
 Error bound, per element:  |C - C_fp64| <= C_GEMM * (|A| @ |W|^T + |b|)  (+ C_TANH absolute after a tanh), so small
 operands cannot hide an error.  C_GEMM is 3x the worst value measured on an H100 80GB HBM3 (400 W power limit) over
@@ -194,6 +195,30 @@ def test_gemm_tc_persistent_tile_counts(bn, extra):
     ref, scale, _ = _ref(A, W, b, 0)
     c = _c(Cout, ref, scale, 0)
     assert c <= C_GEMM, (tiles, c)
+
+
+def _check_epilogue_instance(M, N, K, act, bn, out, seed):
+    """One activation x output-kind instance (out: "f32", "f16" or "both"), activation window [40, N - 24) cutting
+    through a tile: fp32 within the componentwise bound, and the split output exactly the (hi, lo) split of what the
+    fp32 output holds (split alone: hi + lo within the bound after the split's own rounding)."""
+    act_lo, act_hi = 40, N - 24
+    A, W, b = _operands(M, N, K, seed)
+    Cout = torch.full((M, N), float("nan"), device="cuda") if out != "f16" else None
+    hi = torch.zeros((M, N), dtype=torch.float16, device="cuda") if out != "f32" else None
+    lo = torch.zeros_like(hi) if hi is not None else None
+    _gemm(A, W, b, M, N, K, act, bn, out=Cout, split=(hi, lo) if hi is not None else None, ldh=N if hi is not None else 0,
+          act_lo=act_lo, act_hi=act_hi)
+    ref, scale, win = _ref(A, W, b, act, act_lo, act_hi)
+    if Cout is not None:
+        c = _c(Cout, ref, scale, act, win)
+        assert c <= C_GEMM, c
+        if hi is not None:
+            assert _split_ok(hi, lo, Cout)
+    else:
+        s = hi.double() + lo.double()
+        floor = 2.0 ** -22 * ref.abs() + 2.0 ** -25 + (C_TANH * win.double() if act == 2 else 0.0)
+        excess = ((s - ref).abs() - floor).clamp_min(0)
+        assert float((excess / scale.clamp_min(1e-300)).max()) <= C_GEMM
 
 
 # row magnitudes of A from which the split keeps fp32-equivalent accuracy with the fixed 2^6 weight scale

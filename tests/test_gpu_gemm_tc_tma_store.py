@@ -7,7 +7,7 @@ instances.  An output TMA cannot store (unaligned base or row pitch) is refused 
 import pytest
 import torch
 
-from tests.test_gpu_gemm_tc import C_GEMM, _c, _gemm, _lib, _operands, _ref, _split_ok
+from tests.test_gpu_gemm_tc import _check_epilogue_instance, _gemm, _lib, _operands
 
 pytestmark = pytest.mark.gpu
 
@@ -22,26 +22,8 @@ def _rows_for_three_tiles_per_cta(N):
 @pytest.mark.parametrize("out", ["f32", "f16", "both"])
 @pytest.mark.parametrize("act", [0, 1, 2])
 def test_gemm_tc_bn256_staging_reused_across_tiles(act, out):
-    N, K = 512, 128
-    M = _rows_for_three_tiles_per_cta(N)
-    act_lo, act_hi = 40, N - 24
-    A, W, b = _operands(M, N, K, 900 + 3 * act + len(out))
-    Cout = torch.full((M, N), float("nan"), device="cuda") if out != "f16" else None
-    hi = torch.zeros((M, N), dtype=torch.float16, device="cuda") if out != "f32" else None
-    lo = torch.zeros_like(hi) if hi is not None else None
-    _gemm(A, W, b, M, N, K, act, 256, out=Cout, split=(hi, lo) if hi is not None else None,
-          ldh=N if hi is not None else 0, act_lo=act_lo, act_hi=act_hi)
-    ref, scale, win = _ref(A, W, b, act, act_lo, act_hi)
-    if Cout is not None:
-        c = _c(Cout, ref, scale, act, win)
-        assert c <= C_GEMM, c
-        if hi is not None:
-            assert _split_ok(hi, lo, Cout)
-    else:
-        s = hi.double() + lo.double()
-        floor = 2.0 ** -22 * ref.abs() + 2.0 ** -25 + (1e-6 * win.double() if act == 2 else 0.0)
-        excess = ((s - ref).abs() - floor).clamp_min(0)
-        assert float((excess / scale.clamp_min(1e-300)).max()) <= C_GEMM
+    N = 512
+    _check_epilogue_instance(_rows_for_three_tiles_per_cta(N), N, 128, act, 256, out, 900 + 3 * act + len(out))
 
 
 @pytest.mark.parametrize("case", ["f32_base", "f16_base", "f16_pitch"])

@@ -1,9 +1,9 @@
 """Where the time of one tile of the BN = 256 tensor-core GEMM goes: per-tile timestamps from a traced build.
 
-Compiles cn_policy.cu with -DCN_GEMM_TRACE (the repository's nvcc flags otherwise) into a separate library in a
-temporary directory; the default build has no trace code.  In the traced build consumer warp 0 of every CTA records,
-for each tile, %globaltimer at the tile start, at the first pass of a full barrier (operands landed), at the end of the
-main loop and at the end of the epilogue (the moment it handed the tile's last output box to TMA), counts its failed
+Compiles the GEMM unit cn_gemm_tc.cu (with cn_host_util.cpp, the error plumbing it links against) with -DCN_GEMM_TRACE
+(the repository's nvcc flags otherwise) into a separate library in a temporary directory; the default build has no
+trace code.  In the traced build consumer warp 0 of every CTA records, for each tile, %globaltimer at the tile start,
+at the first pass of a full barrier (operands landed), at the end of the main loop and at the end of the epilogue (the moment it handed the tile's last output box to TMA), counts its failed
 polls of the full barriers, and counts the waits for a staging buffer whose previous box TMA had not yet read
 (cn_gemm_tc.cuh, TC_TRACE_REC).
 
@@ -38,7 +38,7 @@ GEMMS = [("embed2", 128, 512, 1, "f16"), ("qkv", 512, 1536, 0, "f32"), ("outproj
 def build(out):
     from __graft_entry__ import ARCH, COMMON
     cmd = (["nvcc"] + ARCH + COMMON + ["-DCN_GEMM_TRACE", "-shared", "-o", out,
-                                        os.path.join(CSRC, "cn_policy.cu"), os.path.join(CSRC, "cn_host_util.cpp")])
+                                        os.path.join(CSRC, "cn_gemm_tc.cu"), os.path.join(CSRC, "cn_host_util.cpp")])
     subprocess.check_call(cmd)
     return out
 
