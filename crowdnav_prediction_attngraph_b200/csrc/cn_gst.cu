@@ -1,5 +1,4 @@
-// BASELINE config 3 (SURVEY.md row a16): the GST trajectory predictor and the VecPretextNormalize processing,
-// fused into ONE kernel launch per rollout step.
+// BASELINE config 3 (SURVEY.md row a16): the GST trajectory predictor and the VecPretextNormalize processing.
 //
 //   reference: rl/vec_env/vec_pretext_normalize.py:85-191 (traj / mask deques, process_obs_rew),
 //              gst_updated/scripts/wrapper/crowd_nav_interface_parallel.py:45-114 (input masks, cumsum of mu),
@@ -7,307 +6,82 @@
 //              mha.py:236-242 for the shipped predictor configuration (full connectivity, one 8-head layer,
 //              'faster_lstm', recursive decoding, sampling=False).
 //
-// One CTA per environment: the five observed frames are stacked as 5*H rows so every weight matrix of the encoder
-// layer is read once for them, the LSTM runs its five steps on the H nodes, four more encoder + LSTM steps decode
-// the future, and the CTA finishes the wrapper's work: future-collision penalty added to the reward, predicted
-// relative positions written into the 2(P+1)-wide spatial_edges rows, rows sorted by distance to the robot.
-// All activations live in shared memory; weights are stored transposed ([K][N]) so the register-tiled dense
-// layers read them coalesced (they stay L2 resident: 269 KB).  fp32 CUDA cores: this first version favours
-// parity (<= 2e-5 on the predicted positions).  The default path since is cn_gst_tc.cu (batched wgmma GEMMs over
-// all environments + row-wise kernels); this fused kernel stays as CN_GST_MODE=fused (one launch, no workspace).
+// Every dense layer is a batched [rows, K] GEMM over ALL environments on the wgmma 3xFP16 GEMM (cn_gemm_tc.h), over
+// the rows whose mask is 1 only (see the compact-row comment below), and small row-wise kernels do embedding +
+// LayerNorm, the H x H attention, residuals, the LSTM cell and the wrapper's tail: future-collision penalty added to the
+// reward, predicted relative positions written into the 2(P+1)-wide spatial_edges rows, rows sorted by distance to the
+// robot.  The launches of one step form a chain with programmatic dependent launch (cn_launch.cuh).
 #include <cuda_runtime.h>
-#include <math.h>
 #include <stdint.h>
-#include <stdlib.h>
 #include <string.h>
 #include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/crowdnav_b200.h"
+#include "cn_gemm_tc.h"
 #include "cn_host_util.h"
+#include "cn_launch.cuh"
 
 namespace {
 
-#define GST_D 64
-#define GST_T 5          // observed frames = predicted steps
-#define GST_THREADS 1024
-#define GST_INVALID (-999.0f)
+#define GT_T 5
+#define GT_INVALID (-999.0f)
 
-struct GstW {
-  const float *We_t, *be, *ln0_g, *ln0_b, *Win_t, *bin, *Wout_t, *bout, *ln1_g, *ln1_b;
-  const float *W1_t, *b1, *W2_t, *b2, *Wih_t, *bih, *Whh_t, *bhh, *Wp, *bp;
+struct GstTcW {   // fp32 device parameters used by the row-wise kernels
+  const float *We_t, *be, *ln0_g, *ln0_b, *ln1_g, *ln1_b, *Wp, *bp;
+  const float *bin, *bout, *b1, *b2, *bih, *bhh;
 };
 
-// out[r][c] = act(res[r][c] + bias[c] + sum_k in[r][k] * Wt[k][c]); RT x 4 register tiles, column tiles fastest
-// across the threads (coalesced float4 weight loads, broadcast activation loads).  R % RT == 0, Nout % 4 == 0.
-template <int RT>
-__device__ void gst_dense_t(const float* __restrict__ in, int ldi, const float* __restrict__ Wt, const float* __restrict__ bias,
-                            const float* res, int ldr, float* out, int ldo, int R, int K, int Nout, bool relu) {
-  const int ct = Nout >> 2, rt = R / RT;
-  for (int tile = threadIdx.x; tile < ct * rt; tile += blockDim.x) {
-    const int c0 = (tile % ct) << 2, r0 = (tile / ct) * RT;
-    float acc[RT][4];
-    const float4 b = *reinterpret_cast<const float4*>(bias + c0);
-#pragma unroll
-    for (int i = 0; i < RT; ++i) { acc[i][0] = b.x; acc[i][1] = b.y; acc[i][2] = b.z; acc[i][3] = b.w; }
-    const float* ip = in + (size_t)r0 * ldi;
-    for (int k = 0; k < K; k += 4) {                       // K % 4 == 0; activations fetched as LDS.128 over k
-      float4 wv[4];
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wv[kk] = __ldg(reinterpret_cast<const float4*>(Wt + (size_t)(k + kk) * Nout + c0));
-#pragma unroll
-      for (int i = 0; i < RT; ++i) {
-        const float4 a4 = *reinterpret_cast<const float4*>(ip + i * ldi + k);
-        const float a[4] = {a4.x, a4.y, a4.z, a4.w};
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          acc[i][0] = fmaf(a[kk], wv[kk].x, acc[i][0]); acc[i][1] = fmaf(a[kk], wv[kk].y, acc[i][1]);
-          acc[i][2] = fmaf(a[kk], wv[kk].z, acc[i][2]); acc[i][3] = fmaf(a[kk], wv[kk].w, acc[i][3]);
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < RT; ++i) {
-      float4 v = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
-      if (res) {
-        const float4 r = *reinterpret_cast<const float4*>(res + (size_t)(r0 + i) * ldr + c0);
-        v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
-      }
-      if (relu) { v.x = fmaxf(v.x, 0.0f); v.y = fmaxf(v.y, 0.0f); v.z = fmaxf(v.z, 0.0f); v.w = fmaxf(v.w, 0.0f); }
-      *reinterpret_cast<float4*>(out + (size_t)(r0 + i) * ldo + c0) = v;
-    }
-  }
-}
-// tile height chosen so that (almost) every thread of the CTA gets a tile
-__device__ void gst_dense(const float* __restrict__ in, int ldi, const float* __restrict__ Wt, const float* __restrict__ bias,
-                          const float* res, int ldr, float* out, int ldo, int R, int K, int Nout, bool relu) {
-  const int ct = Nout >> 2;
-  if ((R >> 2) * ct >= (int)blockDim.x) gst_dense_t<4>(in, ldi, Wt, bias, res, ldr, out, ldo, R, K, Nout, relu);
-  else if ((R >> 1) * ct >= (int)blockDim.x) gst_dense_t<2>(in, ldi, Wt, bias, res, ldr, out, ldo, R, K, Nout, relu);
-  else gst_dense_t<1>(in, ldi, Wt, bias, res, ldr, out, ldo, R, K, Nout, relu);
+__device__ __forceinline__ void gt_split_store(__half* hi, __half* lo, size_t idx, float x) {
+  const float c = fminf(fmaxf(x, -65504.0f), 65504.0f);
+  const __half h = __float2half_rn(c);
+  hi[idx] = h;
+  lo[idx] = __float2half_rn(c - __half2float(h));
 }
 
-// LayerNorm over the 64 features of every row (one warp per row, two features per lane), optional row mask.
-__device__ void gst_layernorm(const float* in, float* out, int R, const float* __restrict__ g, const float* __restrict__ b,
-                              const float* rowmask) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  for (int r = warp; r < R; r += nw) {
-    const float a0 = in[r * GST_D + lane], a1 = in[r * GST_D + lane + 32];
-    float s = a0 + a1;
+// LayerNorm of one 64-wide row held as two values per lane
+__device__ __forceinline__ void gt_ln(float a0, float a1, const float* g, const float* b, int lane, float& o0, float& o1) {
+  float s = a0 + a1;
 #pragma unroll
-    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float mean = s * (1.0f / GST_D);
-    const float d0 = a0 - mean, d1 = a1 - mean;
-    float v = d0 * d0 + d1 * d1;
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float mean = s * (1.0f / 64.0f);
+  const float d0 = a0 - mean, d1 = a1 - mean;
+  float v = d0 * d0 + d1 * d1;
 #pragma unroll
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    const float inv = rsqrtf(v * (1.0f / GST_D) + 1e-5f);
-    const float m = rowmask ? rowmask[r] : 1.0f;
-    out[r * GST_D + lane] = (d0 * inv * g[lane] + b[lane]) * m;
-    out[r * GST_D + lane + 32] = (d1 * inv * g[lane + 32] + b[lane + 32]) * m;
-  }
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const float inv = rsqrtf(v * (1.0f / 64.0f) + 1e-5f);
+  o0 = d0 * inv * g[lane] + b[lane];
+  o1 = d1 * inv * g[lane + 32] + b[lane + 32];
 }
 
-// One node-encoder layer on R = G * H rows (G groups of H nodes attend within their group).
-//   xin  [R][2]   displacements            rowm [R]  node validity (attn_mask[i][j] = rowm[i] * rowm[j])
-//   X    [R][64]  work / result            Y    [R][64] work        BIG [R][192 | 128] work
-__device__ void gst_encoder(const GstW& w, const float* xin, const float* rowm, float* X, float* Y, float* BIG, int R, int H) {
-  // node embedding (K = 2) fused with norm_node and the pedestrian mask
-  for (int i = threadIdx.x; i < R * GST_D; i += blockDim.x) {
-    const int r = i >> 6, c = i & 63;
-    Y[i] = fmaf(xin[2 * r + 1], w.We_t[GST_D + c], fmaf(xin[2 * r], w.We_t[c], w.be[c]));
-  }
-  __syncthreads();
-  gst_layernorm(Y, X, R, w.ln0_g, w.ln0_b, rowm);
-  __syncthreads();
-  gst_dense(X, GST_D, w.Win_t, w.bin, nullptr, 0, BIG, 192, R, GST_D, 192, false);
-  __syncthreads();
-  // attention: one thread per (row, head); soft-max over ALL H neighbours, then mask and renormalise (mha.py:236-242)
-  for (int i = threadIdx.x; i < R * 8; i += blockDim.x) {
-    const int r = i >> 3, hd = i & 7;
-    const int g0 = (r / H) * H;
-    const float scaling = 0.35355339059327373f;       // 8 ** -0.5
-    float q[8];
-#pragma unroll
-    for (int d = 0; d < 8; ++d) q[d] = BIG[r * 192 + hd * 8 + d] * scaling;
-    float mx = -INFINITY;
-    for (int j = 0; j < H; ++j) {
-      const float* kj = BIG + (g0 + j) * 192 + 64 + hd * 8;
-      float s = 0.0f;
-#pragma unroll
-      for (int d = 0; d < 8; ++d) s = fmaf(q[d], kj[d], s);
-      mx = fmaxf(mx, s);
-    }
-    float den = 0.0f, dm = 0.0f, o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const float mi = rowm[r];
-    for (int j = 0; j < H; ++j) {
-      const float* kj = BIG + (g0 + j) * 192 + 64 + hd * 8;
-      const float* vj = BIG + (g0 + j) * 192 + 128 + hd * 8;
-      float s = 0.0f;
-#pragma unroll
-      for (int d = 0; d < 8; ++d) s = fmaf(q[d], kj[d], s);
-      const float e = expf(s - mx);
-      den += e;
-      const float em = e * (mi * rowm[g0 + j]);
-      dm += em;
-#pragma unroll
-      for (int d = 0; d < 8; ++d) o[d] = fmaf(em, vj[d], o[d]);
-    }
-    // w = softmax * mask; w /= (sum(w) + 1e-10)  ==  (e*m/den) / (dm/den + 1e-10)
-    const float scale = (1.0f / den) / (dm / den + 1e-10f);
-#pragma unroll
-    for (int d = 0; d < 8; ++d) Y[r * GST_D + hd * 8 + d] = o[d] * scale;
-  }
-  __syncthreads();
-  gst_dense(Y, GST_D, w.Wout_t, w.bout, X, GST_D, X, GST_D, R, GST_D, GST_D, false);      // x = x + out_proj(attn)
-  __syncthreads();
-  gst_layernorm(X, Y, R, w.ln1_g, w.ln1_b, nullptr);
-  __syncthreads();
-  gst_dense(Y, GST_D, w.W1_t, w.b1, nullptr, 0, BIG, 128, R, GST_D, 128, true);
-  __syncthreads();
-  gst_dense(BIG, 128, w.W2_t, w.b2, X, GST_D, X, GST_D, R, 128, GST_D, false);             // x = x + ffn(norm1(x))
-  __syncthreads();
-}
+__device__ __forceinline__ float gt_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-__device__ __forceinline__ float gst_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
-
-struct GstShared {
-  float* X; float* Y; float* BIG; float* GH;      // [R][64], [R][64], [R][256], [H][256]
-  float* h; float* c;                             // [H][64]
-  float* xin;                                     // [R][2]
-  float* rowm;                                    // [R]
-  float* pos_last; float* mu_cum; float* fp;      // [H][2], [H][2], [H]
-  float* pred;                                    // [H][GST_T][2] predicted world positions
-};
-
-// smem floats needed for H nodes
-__host__ __device__ inline size_t gst_smem_floats(int H) {
-  const size_t R = (size_t)GST_T * H;
-  return R * 64 * 2 + R * 256 + (size_t)H * 256 + (size_t)H * 64 * 2 + R * 2 + R + (size_t)H * (2 + 2 + 1) + (size_t)H * GST_T * 2 + 64;
-}
-
-__global__ void __launch_bounds__(GST_THREADS) cn_pretext_kernel(GstW w, int N, int H, int P, float thr, float collision_penalty,
-                                                                 float* __restrict__ ring_pos /* [5][N][H][2] */,
-                                                                 uint8_t* __restrict__ ring_mask /* [5][N][H] */, int newest,
-                                                                 const float* __restrict__ robot_node /* [N][7] */,
-                                                                 const float* __restrict__ sp2 /* [N][H][2] */,
-                                                                 const uint8_t* __restrict__ vis /* [N][H] */,
-                                                                 float* __restrict__ reward /* [N] or null */,
-                                                                 float* __restrict__ penalty_out /* [N] or null */,
-                                                                 float* __restrict__ out_sp /* [N][H][2(P+1)] */) {
-  extern __shared__ __align__(16) float sm[];
+// process_obs_rew tail: one CTA (32 threads) per environment
+__global__ void __launch_bounds__(32) gt_final_kernel(int N, int H, int P, float thr, float collision_penalty,
+                                                      const float* __restrict__ robot, const float* __restrict__ sp2,
+                                                      const float* __restrict__ fp, const float* __restrict__ pred,
+                                                      float* __restrict__ reward, float* __restrict__ penalty_out,
+                                                      float* __restrict__ out_sp) {
+  cn_pdl_prologue();
   const int e = blockIdx.x;
-  if (e >= N) return;
-  const int R = GST_T * H;
-  GstShared s;
-  float* q = sm;
-  s.X = q; q += R * 64; s.Y = q; q += R * 64; s.BIG = q; q += R * 256; s.GH = q; q += H * 256;
-  s.h = q; q += H * 64; s.c = q; q += H * 64; s.xin = q; q += R * 2; s.rowm = q; q += R;
-  s.pos_last = q; q += H * 2; s.mu_cum = q; q += H * 2; s.fp = q; q += H; s.pred = q;
-  const float rx = robot_node[e * 7], ry = robot_node[e * 7 + 1];
-  // ---- traj_buffer.append(robot + spatial_edges[:, :2]); mask_buffer.append(visible_masks)
-  for (int i = threadIdx.x; i < H; i += blockDim.x) {
-    const size_t o = ((size_t)newest * N + e) * H + i;
-    ring_pos[2 * o] = rx + sp2[((size_t)e * H + i) * 2];
-    ring_pos[2 * o + 1] = ry + sp2[((size_t)e * H + i) * 2 + 1];
-    ring_mask[o] = vis[(size_t)e * H + i] ? 1 : 0;
-  }
-  __syncthreads();
-  // ---- interface.forward input processing: frames oldest -> newest
-  for (int i = threadIdx.x; i < R; i += blockDim.x) {
-    const int t = i / H, n = i - t * H;
-    const int slot = (newest + 1 + t) % GST_T, slot_prev = (newest + t) % GST_T, slot_last = newest;
-    const size_t o = ((size_t)slot * N + e) * H + n, op = ((size_t)slot_prev * N + e) * H + n,
-                 ol = ((size_t)slot_last * N + e) * H + n;
-    // loss_mask_rel_obs: frame 0 = mask[0]; frame t >= 1 = mask[t-1] * mask[LAST] (sic, interface.forward:77-78)
-    const float m = t == 0 ? (float)ring_mask[o] : (float)ring_mask[op] * (float)ring_mask[ol];
-    float dx = 0.0f, dy = 0.0f;
-    if (t > 0) { dx = ring_pos[2 * o] - ring_pos[2 * op]; dy = ring_pos[2 * o + 1] - ring_pos[2 * op + 1]; }
-    s.xin[2 * i] = GST_INVALID * (1.0f - m) + dx * m;
-    s.xin[2 * i + 1] = GST_INVALID * (1.0f - m) + dy * m;
-    s.rowm[i] = m;
-    if (t == GST_T - 1) { s.fp[n] = m; s.pos_last[2 * n] = ring_pos[2 * o]; s.pos_last[2 * n + 1] = ring_pos[2 * o + 1]; }
-  }
-  for (int i = threadIdx.x; i < H * 64; i += blockDim.x) { s.h[i] = 0.0f; s.c[i] = 0.0f; }
-  for (int i = threadIdx.x; i < H * 2; i += blockDim.x) s.mu_cum[i] = 0.0f;
-  __syncthreads();
-  // ---- observation period: encoder on the 5 stacked frames, mask, LSTM
-  gst_encoder(w, s.xin, s.rowm, s.X, s.Y, s.BIG, R, H);
-  for (int i = threadIdx.x; i < R * 64; i += blockDim.x) s.X[i] *= s.rowm[i >> 6];
-  __syncthreads();
-  gst_dense(s.X, GST_D, w.Wih_t, w.bih, nullptr, 0, s.BIG, 256, R, GST_D, 256, false);      // W_ih x_t + b_ih, all frames
-  __syncthreads();
-  for (int t = 0; t < GST_T; ++t) {
-    gst_dense(s.h, GST_D, w.Whh_t, w.bhh, nullptr, 0, s.GH, 256, H, GST_D, 256, false);
-    __syncthreads();
-    for (int i = threadIdx.x; i < H * 64; i += blockDim.x) {
-      const int n = i >> 6, j = i & 63;
-      const float* gx = s.BIG + (size_t)(t * H + n) * 256;
-      const float* gh = s.GH + (size_t)n * 256;
-      const float ig = gst_sigmoid(gx[j] + gh[j]), fg = gst_sigmoid(gx[64 + j] + gh[64 + j]);
-      const float gg = tanhf(gx[128 + j] + gh[128 + j]), og = gst_sigmoid(gx[192 + j] + gh[192 + j]);
-      const float c2 = fg * s.c[i] + ig * gg;
-      s.c[i] = c2; s.h[i] = og * tanhf(c2);
+  const float rx = robot[e * 7], ry = robot[e * 7 + 1];
+  float pen = 0.0f;
+  for (int i = threadIdx.x; i < H * GT_T; i += 32) {
+    const int n = i / GT_T, k = i - n * GT_T;
+    if (k < P && fp[(size_t)e * H + n] != 0.0f) {
+      const float dx = pred[((size_t)e * H * GT_T + i) * 2] - rx, dy = pred[((size_t)e * H * GT_T + i) * 2 + 1] - ry;
+      if (sqrtf(dx * dx + dy * dy) < thr) pen = fminf(pen, collision_penalty / (float)(4 << k));
     }
-    __syncthreads();
   }
-  for (int i = threadIdx.x; i < H * 64; i += blockDim.x) { const float m = s.fp[i >> 6]; s.h[i] *= m; s.c[i] *= m; }
-  __syncthreads();
-  // ---- prediction period (recursive decoding, the mean is fed back)
-  for (int tt = 0; tt < GST_T; ++tt) {
-    if (tt > 0) {
-      gst_encoder(w, s.xin, s.fp, s.X, s.Y, s.BIG, H, H);            // xin = masked mean of the previous step
-      for (int i = threadIdx.x; i < H * 64; i += blockDim.x) s.X[i] *= s.fp[i >> 6];
-      __syncthreads();
-      gst_dense(s.X, GST_D, w.Wih_t, w.bih, nullptr, 0, s.BIG, 256, H, GST_D, 256, false);
-      gst_dense(s.h, GST_D, w.Whh_t, w.bhh, nullptr, 0, s.GH, 256, H, GST_D, 256, false);
-      __syncthreads();
-      for (int i = threadIdx.x; i < H * 64; i += blockDim.x) {
-        const int n = i >> 6, j = i & 63;
-        const float* gx = s.BIG + (size_t)n * 256;
-        const float* gh = s.GH + (size_t)n * 256;
-        const float ig = gst_sigmoid(gx[j] + gh[j]), fg = gst_sigmoid(gx[64 + j] + gh[64 + j]);
-        const float gg = tanhf(gx[128 + j] + gh[128 + j]), og = gst_sigmoid(gx[192 + j] + gh[192 + j]);
-        const float c2 = fg * s.c[i] + ig * gg, h2 = og * tanhf(c2);
-        const float m = s.fp[n];
-        s.c[i] = c2 * m + s.c[i] * (1.0f - m);
-        s.h[i] = h2 * m + s.h[i] * (1.0f - m);
-      }
-      __syncthreads();
-    }
-    // hidden2pos: only the mean is consumed downstream (sigma / corr are dropped by process_obs_rew)
-    for (int i = threadIdx.x; i < H * 2; i += blockDim.x) {
-      const int n = i >> 1, d = i & 1;
-      float a = w.bp[d];
-      for (int k = 0; k < 64; ++k) a = fmaf(s.h[n * 64 + k], w.Wp[d * 64 + k], a);
-      const float m = s.fp[n];
-      s.xin[i] = a * m;                                               // x_sample (masked) = next encoder input
-      const float cum = s.mu_cum[i] + a;
-      s.mu_cum[i] = cum;
-      s.pred[(n * GST_T + tt) * 2 + d] = (cum + s.pos_last[i]) * m + GST_INVALID * (1.0f - m);
-    }
-    __syncthreads();
-  }
-  // ---- process_obs_rew: future-collision penalty, predicted relative positions, sort by distance
-  if (threadIdx.x < 32) {
-    float pen = 0.0f;
-    for (int i = threadIdx.x; i < H * GST_T; i += 32) {
-      const int n = i / GST_T, k = i - n * GST_T;
-      if (k < P && s.fp[n] != 0.0f) {
-        const float dx = s.pred[i * 2] - rx, dy = s.pred[i * 2 + 1] - ry;
-        if (sqrtf(dx * dx + dy * dy) < thr) pen = fminf(pen, collision_penalty / (float)(4 << k));
-      }
-    }
 #pragma unroll
-    for (int o = 16; o; o >>= 1) pen = fminf(pen, __shfl_xor_sync(0xffffffffu, pen, o));
-    if (threadIdx.x == 0) {
-      if (reward) reward[e] += pen;
-      if (penalty_out) penalty_out[e] = pen;
-    }
+  for (int o = 16; o; o >>= 1) pen = fminf(pen, __shfl_xor_sync(0xffffffffu, pen, o));
+  if (threadIdx.x == 0) {
+    if (reward) reward[e] += pen;
+    if (penalty_out) penalty_out[e] = pen;
   }
   const int W = 2 * (P + 1);
-  for (int n = threadIdx.x; n < H; n += blockDim.x) {
+  for (int n = threadIdx.x; n < H; n += 32) {
     const float cx = sp2[((size_t)e * H + n) * 2], cy = sp2[((size_t)e * H + n) * 2 + 1];
     const float key = sqrtf(cx * cx + cy * cy);
     int rank = 0;
@@ -318,12 +92,280 @@ __global__ void __launch_bounds__(GST_THREADS) cn_pretext_kernel(GstW w, int N, 
     }
     float* dst = out_sp + ((size_t)e * H + rank) * W;
     dst[0] = cx; dst[1] = cy;
-    const bool ok = s.fp[n] != 0.0f;
+    const bool ok = fp[(size_t)e * H + n] != 0.0f;
     for (int k = 0; k < P; ++k) {
-      // unpredicted humans keep the tiled current relative position (crowd_sim_pred_real_gst.py generate_ob)
-      dst[2 + 2 * k] = ok ? s.pred[(n * GST_T + k) * 2] - rx : cx;
-      dst[3 + 2 * k] = ok ? s.pred[(n * GST_T + k) * 2 + 1] - ry : cy;
+      dst[2 + 2 * k] = ok ? pred[(((size_t)e * H + n) * GT_T + k) * 2] - rx : cx;
+      dst[3 + 2 * k] = ok ? pred[(((size_t)e * H + n) * GT_T + k) * 2 + 1] - ry : cy;
     }
+  }
+}
+
+// ==========================================================================================================
+// Compact rows.  Every row-wise quantity of the predictor is multiplied by a 0/1 mask: the node embedding by
+// the row's input mask, attention weights by the query's and the key's mask (a masked query's output is exactly 0, a
+// masked key has weight exactly 0), the encoder output by the row mask again before W_ih, the LSTM state by the
+// "visible in the newest frame" flag fp after the observation period and in every decoding step, the prediction by fp.
+// So a masked row carries constants (its Q|K|V row is the bias, its W_ih input is 0 -> its gate pre-activation is
+// b_ih) and a human with fp = 0 carries nothing at all.  With the robot seeing ~4.4 of 20 humans, 78 % of the
+// N*5*H observation rows and of the N*H decoding rows are such constants.  Here only the valid rows exist:
+//   observation period: rows with mask 1, compacted in (env, frame) group order  (count counts[0], group g = e*5+t owns
+//                       compact rows [gstart[g], gstart[g+1]))
+//   LSTM + decoding:    humans with fp = 1, compacted in env order             (count counts[1], env e owns [estart[e], ..))
+// The only place masked rows enter a valid row's arithmetic is the soft-max denominator (soft-max over ALL H neighbours,
+// then mask and renormalise, mha.py:236-242): all masked keys share the key vector b_k, so their H - n terms are
+// (H - n) * exp(q . b_k - max).  Results equal a computation over every row up to the order of that sum (~1e-9
+// relative).  gtc_attn_kernel stages the Q|K|V rows of one group in shared memory: at most GT_MAXH humans.
+#define GT_MAXH 32
+#define GTC_WARPS 8
+
+// one warp per (env, frame) group, lane = human: masks, masked input displacement, group counts, newest-frame bookkeeping
+__global__ void __launch_bounds__(GTC_WARPS * 32) gtc_prep_kernel(int N, int H, float* __restrict__ ring_pos, uint8_t* __restrict__ ring_mask,
+                                                                   int newest, const float* __restrict__ robot, const float* __restrict__ sp2,
+                                                                   const uint8_t* __restrict__ vis, float* __restrict__ rowm,
+                                                                   float* __restrict__ inp, int* __restrict__ gcount,
+                                                                   int* __restrict__ ecount, float* __restrict__ fp,
+                                                                   float* __restrict__ pos_last) {
+  cn_pdl_prologue();
+  const int lane = threadIdx.x & 31;
+  const int g = blockIdx.x * GTC_WARPS + (threadIdx.x >> 5);
+  if (g >= N * GT_T) return;
+  const int e = g / GT_T, t = g - e * GT_T, n = lane;
+  bool valid = false, vnow = false;
+  if (n < H) {
+    auto frame_pos = [&](int tt, float& x, float& y, float& m) {
+      if (tt == GT_T - 1) {
+        x = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
+        y = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
+        m = vis[(size_t)e * H + n] ? 1.0f : 0.0f;
+      } else {
+        const int slot = (newest + 1 + tt) % GT_T;
+        const size_t o = ((size_t)slot * N + e) * H + n;
+        x = ring_pos[2 * o]; y = ring_pos[2 * o + 1]; m = (float)ring_mask[o];
+      }
+    };
+    float x, y, m, xp = 0, yp = 0, mp = 0, xl_, yl_, ml_;
+    frame_pos(t, x, y, m);
+    frame_pos(GT_T - 1, xl_, yl_, ml_);
+    if (t > 0) frame_pos(t - 1, xp, yp, mp);
+    const float mrel = t == 0 ? m : mp * ml_;                  // interface.forward:77-78 (sic)
+    const float dx = t == 0 ? 0.0f : x - xp, dy = t == 0 ? 0.0f : y - yp;
+    const size_t r = (size_t)g * H + n;
+    rowm[r] = mrel;
+    inp[2 * r] = GT_INVALID * (1.0f - mrel) + dx * mrel;
+    inp[2 * r + 1] = GT_INVALID * (1.0f - mrel) + dy * mrel;
+    valid = mrel != 0.0f;
+    if (t == GT_T - 1) {
+      const size_t rd = (size_t)e * H + n;
+      fp[rd] = mrel; pos_last[2 * rd] = x; pos_last[2 * rd + 1] = y;
+      vnow = valid;
+    }
+  }
+  const uint32_t b = __ballot_sync(0xffffffffu, valid);
+  if (lane == 0) gcount[g] = __popc(b);
+  if (t == GT_T - 1) {
+    const uint32_t bn = __ballot_sync(0xffffffffu, vnow);
+    if (lane == 0) ecount[e] = __popc(bn);
+    // traj_buffer.append / mask_buffer.append.  Other groups of this launch read the newest frame from the observation,
+    // never from this slot (frame_pos), so the write cannot race with them.
+    if (n < H) {
+      const size_t o = ((size_t)newest * N + e) * H + n;
+      ring_pos[2 * o] = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
+      ring_pos[2 * o + 1] = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
+      ring_mask[o] = vis[(size_t)e * H + n] ? 1 : 0;
+    }
+  }
+}
+
+// exclusive prefix sums of the group counts (G) and of the per-env visible counts (N); totals -> counts[0], counts[1]
+__global__ void __launch_bounds__(1024) gtc_scan_kernel(const int* __restrict__ gcount, int G, int* __restrict__ gstart,
+                                                        const int* __restrict__ ecount, int N, int* __restrict__ estart,
+                                                        int* __restrict__ counts) {
+  cn_pdl_prologue();
+  __shared__ int part[1024];
+  for (int pass = 0; pass < 2; ++pass) {
+    const int* in = pass ? ecount : gcount;
+    int* out = pass ? estart : gstart;
+    const int L = pass ? N : G;
+    const int per = (L + 1023) / 1024, b0 = threadIdx.x * per;
+    int s = 0;
+    for (int i = b0; i < b0 + per && i < L; ++i) s += in[i];
+    part[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {                      // Hillis-Steele inclusive scan of the 1024 partials
+      const int v = threadIdx.x >= o ? part[threadIdx.x - o] : 0;
+      __syncthreads();
+      part[threadIdx.x] += v;
+      __syncthreads();
+    }
+    int run = part[threadIdx.x] - s;                          // exclusive
+    for (int i = b0; i < b0 + per && i < L; ++i) { out[i] = run; run += in[i]; }
+    if (threadIdx.x == 1023) { out[L] = part[1023]; counts[pass] = part[1023]; }
+    __syncthreads();
+  }
+}
+
+// compaction maps: cidx[r] (compact row or -1), crow[c] (source row), drow[d] (env * H + human of decode row d)
+__global__ void __launch_bounds__(GTC_WARPS * 32) gtc_index_kernel(int N, int H, const float* __restrict__ rowm, const float* __restrict__ fp,
+                                                                    const int* __restrict__ gstart, const int* __restrict__ estart,
+                                                                    int* __restrict__ cidx, int* __restrict__ crow, int* __restrict__ drow) {
+  cn_pdl_prologue();
+  const int lane = threadIdx.x & 31;
+  const int g = blockIdx.x * GTC_WARPS + (threadIdx.x >> 5);
+  if (g >= N * GT_T) return;
+  const int e = g / GT_T, t = g - e * GT_T;
+  const size_t r = (size_t)g * H + lane;
+  const bool valid = lane < H && rowm[r] != 0.0f;
+  const uint32_t b = __ballot_sync(0xffffffffu, valid);
+  const int c = gstart[g] + __popc(b & ((1u << lane) - 1u));
+  if (lane < H) cidx[r] = valid ? c : -1;
+  if (valid) crow[c] = (int)r;
+  if (t == GT_T - 1) {
+    const size_t rd = (size_t)e * H + lane;
+    const bool vnow = lane < H && fp[rd] != 0.0f;
+    const uint32_t bn = __ballot_sync(0xffffffffu, vnow);
+    if (vnow) drow[estart[e] + __popc(bn & ((1u << lane) - 1u))] = (int)rd;
+  }
+}
+
+// node embedding + norm_node of the compact rows (mask == 1).  src: crow (observation period, input from inp[row]) or
+// null (decoding: input = xin[c]).  One warp per row, grid-stride.
+__global__ void __launch_bounds__(256) gtc_embed_kernel(GstTcW w, const int* __restrict__ count, const int* __restrict__ src,
+                                                        const float* __restrict__ in2, float* __restrict__ X0, __half* __restrict__ xh,
+                                                        __half* __restrict__ xl) {
+  cn_pdl_prologue();
+  const int lane = threadIdx.x & 31, C = cn_ld_after_wait(count);
+  for (int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < C; c += (gridDim.x * blockDim.x) >> 5) {
+    const int r = src ? src[c] : c;
+    const float ix = in2[2 * (size_t)r], iy = in2[2 * (size_t)r + 1];
+    const float e0 = fmaf(iy, w.We_t[64 + lane], fmaf(ix, w.We_t[lane], w.be[lane]));
+    const float e1 = fmaf(iy, w.We_t[96 + lane], fmaf(ix, w.We_t[32 + lane], w.be[32 + lane]));
+    float o0, o1;
+    gt_ln(e0, e1, w.ln0_g, w.ln0_b, lane, o0, o1);
+    const size_t b = (size_t)c * 64;
+    X0[b + lane] = o0; X0[b + lane + 32] = o1;
+    gt_split_store(xh, xl, b + lane, o0); gt_split_store(xh, xl, b + lane + 32, o1);
+  }
+}
+
+// attention within a group's compact rows [start[g], start[g+1]); the H - n masked neighbours enter the soft-max
+// denominator through their common key b_k (see the header of this section).  One CTA per group.
+__global__ void __launch_bounds__(8 * GT_MAXH) gtc_attn_kernel(int H, const int* __restrict__ start, const float* __restrict__ qkv,
+                                                               const float* __restrict__ bk /* b_in + 64 */, __half* __restrict__ ah,
+                                                               __half* __restrict__ al) {
+  cn_pdl_prologue();
+  __shared__ __align__(16) float sq[GT_MAXH * 192];
+  const int c0 = cn_ld_after_wait(start + blockIdx.x), ng = cn_ld_after_wait(start + blockIdx.x + 1) - c0;
+  if (ng <= 0) return;
+  for (int i = threadIdx.x; i < ng * 48; i += blockDim.x)
+    reinterpret_cast<float4*>(sq)[i] = __ldg(reinterpret_cast<const float4*>(qkv + (size_t)c0 * 192) + i);
+  __syncthreads();
+  const int lr = threadIdx.x >> 3, hd = threadIdx.x & 7;
+  if (lr >= ng) return;
+  const float scaling = 0.35355339059327373f;
+  float q[8];
+#pragma unroll
+  for (int d = 0; d < 8; ++d) q[d] = sq[lr * 192 + hd * 8 + d] * scaling;
+  const int nmask = H - ng;
+  float sm = 0.0f;
+#pragma unroll
+  for (int d = 0; d < 8; ++d) sm = fmaf(q[d], __ldg(bk + hd * 8 + d), sm);
+  float mx = nmask > 0 ? sm : -INFINITY;
+  for (int j = 0; j < ng; ++j) {
+    const float* kj = sq + j * 192 + 64 + hd * 8;
+    float s = 0.0f;
+#pragma unroll
+    for (int d = 0; d < 8; ++d) s = fmaf(q[d], kj[d], s);
+    mx = fmaxf(mx, s);
+  }
+  float den = 0.0f, dm = 0.0f, o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int j = 0; j < ng; ++j) {
+    const float* kj = sq + j * 192 + 64 + hd * 8;
+    const float* vj = sq + j * 192 + 128 + hd * 8;
+    float s = 0.0f;
+#pragma unroll
+    for (int d = 0; d < 8; ++d) s = fmaf(q[d], kj[d], s);
+    const float ex = expf(s - mx);
+    den += ex;
+    dm += ex;
+#pragma unroll
+    for (int d = 0; d < 8; ++d) o[d] = fmaf(ex, vj[d], o[d]);
+  }
+  if (nmask > 0) den += (float)nmask * expf(sm - mx);
+  const float scale = (1.0f / den) / (dm / den + 1e-10f);
+  const size_t ob = (size_t)(c0 + lr) * 64 + hd * 8;
+#pragma unroll
+  for (int d = 0; d < 8; ++d) gt_split_store(ah, al, ob + d, o[d] * scale);
+}
+
+// X1 = X0 + O, Y = norm1(X1) (compact rows, grid-stride)
+__global__ void __launch_bounds__(256) gtc_res_ln_kernel(GstTcW w, const int* __restrict__ count, const float* __restrict__ X0,
+                                                         const float* __restrict__ O, float* __restrict__ X1, __half* __restrict__ yh,
+                                                         __half* __restrict__ yl) {
+  cn_pdl_prologue();
+  const int lane = threadIdx.x & 31, C = cn_ld_after_wait(count);
+  for (int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < C; c += (gridDim.x * blockDim.x) >> 5) {
+    const size_t b = (size_t)c * 64;
+    const float a0 = X0[b + lane] + O[b + lane], a1 = X0[b + lane + 32] + O[b + lane + 32];
+    X1[b + lane] = a0; X1[b + lane + 32] = a1;
+    float o0, o1;
+    gt_ln(a0, a1, w.ln1_g, w.ln1_b, lane, o0, o1);
+    gt_split_store(yh, yl, b + lane, o0); gt_split_store(yh, yl, b + lane + 32, o1);
+  }
+}
+
+// XS = X1 + O2 (row mask == 1) as fp16 hi / lo
+__global__ void __launch_bounds__(256) gtc_res_kernel(const int* __restrict__ count, const float* __restrict__ X1,
+                                                      const float* __restrict__ O2, __half* __restrict__ sh, __half* __restrict__ sl) {
+  cn_pdl_prologue();
+  const size_t total = (size_t)cn_ld_after_wait(count) * 64;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x)
+    gt_split_store(sh, sl, i, X1[i] + O2[i]);
+}
+
+// LSTM cell over the compact decode rows.  t >= 0: observation frame t, the row's gate input is GX[cidx] or, when that
+// frame of the human is masked, the constant b_ih;  t < 0: decoding, gate input GX[d].  Also initialises (t == 0).
+__global__ void __launch_bounds__(256) gtc_cell_kernel(int H, int t, const int* __restrict__ count, const int* __restrict__ drow,
+                                                       const int* __restrict__ cidx, const float* __restrict__ GX,
+                                                       const float* __restrict__ bih, const float* __restrict__ bhh,
+                                                       const float* __restrict__ GH, float* __restrict__ h32,
+                                                       float* __restrict__ c32, __half* __restrict__ hh, __half* __restrict__ hl) {
+  cn_pdl_prologue();
+  const size_t total = (size_t)cn_ld_after_wait(count) * 64;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int j = (int)(i & 63);
+    const size_t d = i >> 6;
+    const float* gx;
+    if (t >= 0) {
+      const int rd = drow[d], e = rd / H, n = rd - e * H;
+      const int c = cidx[((size_t)e * GT_T + t) * H + n];
+      gx = c >= 0 ? GX + (size_t)c * 256 : bih;
+    } else {
+      gx = GX + d * 256;
+    }
+    const float* gh = t == 0 ? bhh : GH + d * 256;            // h0 = 0: W_hh h + b_hh = b_hh
+    const float cprev = t == 0 ? 0.0f : c32[i];
+    const float ig = gt_sigmoid(gx[j] + gh[j]), fg = gt_sigmoid(gx[64 + j] + gh[64 + j]);
+    const float gg = tanhf(gx[128 + j] + gh[128 + j]), og = gt_sigmoid(gx[192 + j] + gh[192 + j]);
+    const float c2 = fg * cprev + ig * gg, h2 = og * tanhf(c2);
+    c32[i] = c2; h32[i] = h2;
+    gt_split_store(hh, hl, i, h2);
+  }
+}
+
+// hidden2pos (mean only) of the compact decode rows -> next input, cumulative mean, predicted world position
+__global__ void __launch_bounds__(256) gtc_h2p_kernel(GstTcW w, int tt, const int* __restrict__ count, const int* __restrict__ drow,
+                                                      const float* __restrict__ h32, const float* __restrict__ pos_last,
+                                                      float* __restrict__ xin, float* __restrict__ mu_cum, float* __restrict__ pred) {
+  cn_pdl_prologue();
+  const int total = cn_ld_after_wait(count) * 2;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    const int d = i >> 1, dim = i & 1, rd = drow[d];
+    float a = w.bp[dim];
+    for (int k = 0; k < 64; ++k) a = fmaf(h32[(size_t)d * 64 + k], w.Wp[dim * 64 + k], a);
+    xin[i] = a;
+    const float cum = (tt == 0 ? 0.0f : mu_cum[i]) + a;
+    mu_cum[i] = cum;
+    pred[((size_t)rd * GT_T + tt) * 2 + dim] = cum + pos_last[2 * (size_t)rd + dim];
   }
 }
 
@@ -340,84 +382,104 @@ const char* kParamNames[] = {
     "lstm.weight_ih_l0", "lstm.bias_ih_l0", "lstm.weight_hh_l0", "lstm.bias_hh_l0", "hidden2pos.weight", "hidden2pos.bias"};
 const int kParamRows[] = {64, 64, 64, 64, 192, 192, 64, 64, 64, 64, 128, 128, 64, 64, 256, 256, 256, 256, 5, 5};
 const int kParamCols[] = {2, 1, 1, 1, 64, 1, 64, 1, 1, 1, 64, 1, 128, 1, 64, 1, 64, 1, 64, 1};
-const bool kTranspose[] = {true, false, false, false, true, false, true, false, false, false,
-                           true, false, true, false, true, false, true, false, false, false};
 const int kNumParams = 20;
+
+int gt_upload(CnLaunchCtx* ctx, const float** dst, const float* src, size_t count) {
+  float* q = nullptr;
+  int rc = palloc(ctx, &q, count);
+  if (rc) return rc;
+  if (cudaMemcpy(q, src, count * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return cn_set_error("cn_gst_finalize: H2D failed");
+  *dst = q;
+  return 0;
+}
 
 }  // namespace
 
-// tensor-core implementation (cn_gst_tc.cu)
-void* cn_gst_tc_create(int N, int H, int P, float thr, float pen, int device, const float* const* host, const int* rows,
-                       const int* cols);
-void cn_gst_tc_destroy(void* handle);
-int64_t cn_gst_tc_launches(void* handle);
-int cn_gst_tc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newest, const float* robot, const float* sp2,
-                   const uint8_t* vis, float* reward, float* penalty, float* out_sp, cudaStream_t st);
-int cn_gst_tcc_step(void* handle, float* ring_pos, uint8_t* ring_mask, int newest, const float* robot, const float* sp2,
-                    const uint8_t* vis, float* reward, float* penalty, float* out_sp, cudaStream_t st);
-
 struct cn_gst {
-  void* tc;           // non-null: dense layers on the tensor-core GEMM (CN_GST_MODE=tcc (default) or tc)
-  bool compact;       // tcc: only the rows whose mask is 1 are computed (cn_gst_tcc_step)
+  CnLaunchCtx ctx;
+  size_t ws_allocs;   // ctx.allocs[0..ws_allocs) = ring buffers + workspace (kept); the rest = parameters of the last finalize
   int N, H, P, device;
   float thr, collision_penalty;
   std::map<std::string, std::vector<float>> host;
-  std::vector<void*> allocs;
-  const float* dev[kNumParams];
-  float* ring_pos;
-  uint8_t* ring_mask;
-  int newest;         // ring slot of the most recent frame
   bool finalized;
-  int64_t launches;
-  size_t smem;
+  float* ring_pos;    // [5][N][H][2] traj_buffer
+  uint8_t* ring_mask; // [5][N][H] mask_buffer
+  int newest;         // ring slot of the most recent frame
+  GstTcW w;
+  TcMat tWin, tWout, tW1, tW2, tWih, tWhh;                   // weights (x 2^6, fp16 hi/lo)
+  TcMat tX, tA, tY, tF, tXS, tHd;                            // activations (fp16 hi/lo A operands)
+  float *X0, *QKV, *O, *X1, *GX, *GH, *rowm, *fp, *pos_last, *h32, *c32, *mu_cum, *xin, *pred;
+  TcStoreMap GX_R, GX_Rd, GH_Rd;                             // store maps of the BN = 256 gate GEMMs' outputs, per row extent
+  float* inp;                                                // [R, 2] masked input displacement of every (env, frame, human) row
+  int *cidx, *crow, *gcount, *gstart, *ecount, *estart, *drow, *counts;   // compaction maps (see gtc_* kernels)
 };
 
 extern "C" {
+
+int cn_gst_destroy(cn_gst* g) {
+  if (!g) return 0;
+  cudaSetDevice(g->device);
+  cudaDeviceSynchronize();
+  cn_launch_free(&g->ctx);
+  delete g;
+  return 0;
+}
 
 int cn_gst_create(int num_envs, int human_num, int predict_steps, double robot_radius, double human_radius,
                   double collision_penalty, int device, cn_gst** out) {
   if (!out) return cn_set_error("cn_gst_create: null argument");
   *out = nullptr;
-  if (num_envs <= 0 || human_num <= 0 || human_num % 4 || predict_steps < 1 || predict_steps > GST_T)
+  if (num_envs <= 0 || human_num <= 0 || human_num % 4 || predict_steps < 1 || predict_steps > GT_T)
     return cn_set_error("cn_gst_create: need num_envs > 0, human_num %% 4 == 0 and 1 <= predict_steps <= %d (got %d, %d, %d)",
-                        GST_T, num_envs, human_num, predict_steps);
+                        GT_T, num_envs, human_num, predict_steps);
   int ndev = 0;
   cudaError_t err = cudaGetDeviceCount(&ndev);
   if (err != cudaSuccess || ndev == 0)
     return cn_set_error("cn_gst_create: no CUDA device (%s); this engine has no CPU fallback",
                         err == cudaSuccess ? "device count 0" : cudaGetErrorString(err));
   if (device < 0 || device >= ndev) return cn_set_error("cn_gst_create: bad device %d", device);
-  if (human_num > 32) return cn_set_error("cn_gst_create: human_num %d > 32 is not supported by the predictor kernels", human_num);
-  const size_t smem = gst_smem_floats(human_num) * sizeof(float);
-  if (smem > 227 * 1024)
-    return cn_set_error("cn_gst_create: human_num %d needs %zu bytes of shared memory (max 232448)", human_num, smem);
+  // human_num <= 24 is the range the predictor has always accepted: its first implementation ran one CTA per environment
+  // with the five observed frames in shared memory, which holds at most 24 humans.  The kernels of this file would hold
+  // GT_MAXH = 32; a wider range needs tests of its own.
+  if (human_num > 24)
+    return cn_set_error("cn_gst_create: human_num %d > 24 is not supported (the predictor's accepted range, set by the "
+                        "shared memory of its first, one-CTA-per-environment implementation)", human_num);
   cudaSetDevice(device);
   cn_gst* g = new cn_gst();
   g->N = num_envs; g->H = human_num; g->P = predict_steps; g->device = device;
   g->thr = (float)(robot_radius + human_radius); g->collision_penalty = (float)collision_penalty;
-  g->newest = GST_T - 1; g->finalized = false; g->launches = 0; g->smem = smem; g->tc = nullptr; g->compact = true;
-  g->ring_pos = nullptr; g->ring_mask = nullptr;
-  void* q = nullptr;
-  err = cudaMalloc(&q, (size_t)GST_T * num_envs * human_num * 2 * sizeof(float));
-  if (err == cudaSuccess) { g->ring_pos = (float*)q; g->allocs.push_back(q); err = cudaMalloc(&q, (size_t)GST_T * num_envs * human_num); }
-  if (err == cudaSuccess) { g->ring_mask = (uint8_t*)q; g->allocs.push_back(q); }
-  if (err == cudaSuccess) err = cudaFuncSetAttribute(cn_pretext_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (err != cudaSuccess) {
-    for (void* a : g->allocs) cudaFree(a);
-    delete g;
-    return cn_set_error("cn_gst_create: %s", cudaGetErrorString(err));
-  }
+  g->newest = GT_T - 1; g->finalized = false;
+  CnLaunchCtx* ctx = &g->ctx;
+  cn_launch_init(ctx, device);
+  int rc = tc_set_attrs();
+  const size_t R = (size_t)num_envs * GT_T * human_num, Rd = (size_t)num_envs * human_num;
+  float* q = nullptr;
+  if (!rc) rc = palloc(ctx, &g->ring_pos, R * 2);
+  if (!rc) rc = palloc(ctx, &q, (R + 3) / 4);
+  g->ring_mask = reinterpret_cast<uint8_t*>(q);
+  if (!rc) rc = tc_alloc(ctx, g->tX, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tA, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tY, (int)R, 64, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tF, (int)R, 128, TC_BM, tc_box_k(64));
+  if (!rc) rc = tc_alloc(ctx, g->tXS, (int)R, 64, TC_BM, tc_box_k(256));     // A of the BN = 256 gate GEMMs
+  if (!rc) rc = tc_alloc(ctx, g->tHd, (int)Rd, 64, TC_BM, tc_box_k(256));
+#define GA(name, count) if (!rc) rc = palloc(ctx, &g->name, (count))
+  GA(X0, R * 64); GA(QKV, R * 192); GA(O, R * 64); GA(X1, R * 64); GA(GX, R * 256); GA(GH, Rd * 256); GA(rowm, R); GA(fp, Rd);
+  GA(pos_last, Rd * 2); GA(h32, Rd * 64); GA(c32, Rd * 64); GA(mu_cum, Rd * 2); GA(xin, Rd * 2); GA(pred, Rd * GT_T * 2);
+  GA(inp, R * 2);
+#undef GA
+  // the encoder runs over all R observation rows and over the Rd rows of the newest frame: one GX map per row extent
+  if (!rc) rc = make_store_map(&g->GX_R, g->GX, 4, (int)R, 256, 256);
+  if (!rc) rc = make_store_map(&g->GX_Rd, g->GX, 4, (int)Rd, 256, 256);
+  if (!rc) rc = make_store_map(&g->GH_Rd, g->GH, 4, (int)Rd, 256, 256);
+#define GI(name, count) if (!rc) { float* q_ = nullptr; rc = palloc(ctx, &q_, (count)); g->name = reinterpret_cast<int*>(q_); }
+  GI(cidx, R); GI(crow, R); GI(gcount, (size_t)num_envs * GT_T); GI(gstart, (size_t)num_envs * GT_T + 1); GI(ecount, num_envs);
+  GI(estart, num_envs + 1); GI(drow, Rd); GI(counts, 4);
+#undef GI
+  if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = cn_set_error("cn_gst_create: setup failed");
+  if (rc) { cn_gst_destroy(g); return rc; }
+  g->ws_allocs = ctx->allocs.size();
   *out = g;
-  return 0;
-}
-
-int cn_gst_destroy(cn_gst* g) {
-  if (!g) return 0;
-  cudaSetDevice(g->device);
-  cudaDeviceSynchronize();
-  if (g->tc) cn_gst_tc_destroy(g->tc);
-  for (void* a : g->allocs) cudaFree(a);
-  delete g;
   return 0;
 }
 
@@ -438,35 +500,39 @@ int cn_gst_set_param(cn_gst* g, const char* name, const float* data, size_t coun
 
 int cn_gst_finalize(cn_gst* g) {
   if (!g) return cn_set_error("cn_gst_finalize: null argument");
-  cudaSetDevice(g->device);
+  const float* host[kNumParams];
   for (int i = 0; i < kNumParams; ++i) {
     auto it = g->host.find(kParamNames[i]);
     if (it == g->host.end()) return cn_set_error("cn_gst_finalize: parameter '%s' was not set", kParamNames[i]);
-    std::vector<float> v = it->second;
-    const int rows = kParamRows[i], cols = kParamCols[i];
-    if (kTranspose[i]) {                       // [out][in] -> [in][out]
-      std::vector<float> t(v.size());
-      for (int r = 0; r < rows; ++r) for (int c = 0; c < cols; ++c) t[(size_t)c * rows + r] = v[(size_t)r * cols + c];
-      v.swap(t);
-    }
-    void* q = nullptr;
-    cudaError_t err = cudaMalloc(&q, v.size() * sizeof(float));
-    if (err == cudaSuccess) err = cudaMemcpy(q, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice);
-    if (err != cudaSuccess) return cn_set_error("cn_gst_finalize: %s", cudaGetErrorString(err));
-    g->allocs.push_back(q);
-    g->dev[i] = (const float*)q;
+    host[i] = it->second.data();
   }
-  // default: dense layers as batched tensor-core GEMMs over all environments (cn_gst_tc.cu, 2.5x faster at N = 4096);
-  // CN_GST_MODE=fused selects the single fused CUDA-core kernel of this file (no workspace, one launch)
-  const char* mode = getenv("CN_GST_MODE");
-  g->compact = !(mode && strcmp(mode, "tc") == 0);          // default "tcc": compact rows; "tc": every row
-  if (!(mode && strcmp(mode, "fused") == 0)) {
-    if (g->tc) { cn_gst_tc_destroy(g->tc); g->tc = nullptr; }
-    const float* hp[kNumParams];
-    for (int i = 0; i < kNumParams; ++i) hp[i] = g->host[kParamNames[i]].data();
-    g->tc = cn_gst_tc_create(g->N, g->H, g->P, g->thr, g->collision_penalty, g->device, hp, kParamRows, kParamCols);
-    if (!g->tc) return 1;                       // cn_last_error holds the reason
+  cudaSetDevice(g->device);
+  g->finalized = false;
+  // release the device parameters of a previous finalize (ring buffers and workspace come first and stay)
+  CnLaunchCtx* ctx = &g->ctx;
+  cudaDeviceSynchronize();
+  for (size_t i = g->ws_allocs; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
+  ctx->allocs.resize(g->ws_allocs);
+  // indices in kParamNames: 0 We 1 be 2 ln0g 3 ln0b 4 Win 5 bin 6 Wout 7 bout 8 ln1g 9 ln1b 10 W1 11 b1 12 W2 13 b2
+  //                         14 Wih 15 bih 16 Whh 17 bhh 18 Wp 19 bp
+  std::vector<float> wet(128);
+  for (int c = 0; c < 64; ++c) { wet[c] = host[0][c * 2]; wet[64 + c] = host[0][c * 2 + 1]; }     // [64][2] -> [2][64]
+  int rc = gt_upload(ctx, &g->w.We_t, wet.data(), 128);
+  const float** fdst[] = {&g->w.be, &g->w.ln0_g, &g->w.ln0_b, &g->w.bin, &g->w.bout, &g->w.ln1_g, &g->w.ln1_b, &g->w.b1, &g->w.b2,
+                          &g->w.bih, &g->w.bhh, &g->w.Wp, &g->w.bp};
+  const int fidx[] = {1, 2, 3, 5, 7, 8, 9, 11, 13, 15, 17, 18, 19};
+  for (int i = 0; i < 13 && !rc; ++i) rc = gt_upload(ctx, fdst[i], host[fidx[i]], (size_t)kParamRows[fidx[i]] * kParamCols[fidx[i]]);
+  struct { int idx; TcMat* t; } tw[6] = {{4, &g->tWin}, {6, &g->tWout}, {10, &g->tW1}, {12, &g->tW2}, {14, &g->tWih}, {16, &g->tWhh}};
+  for (int i = 0; i < 6 && !rc; ++i) {
+    const int r = kParamRows[tw[i].idx], k = kParamCols[tw[i].idx];
+    const float* d = nullptr;
+    rc = gt_upload(ctx, &d, host[tw[i].idx], (size_t)r * k);
+    const int bn = r == 256 ? 256 : 64;                                       // the 256-wide gate GEMMs use BN = 256 tiles
+    if (!rc) rc = tc_alloc(ctx, *tw[i].t, r, k, bn, tc_box_k(bn));
+    if (!rc) split16(ctx, 0, d, 64.0f, tw[i].t->hi, tw[i].t->lo, (size_t)r * k);
   }
+  if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = cn_set_error("cn_gst_finalize: weight upload failed");
+  if (rc) return rc;
   g->finalized = true;
   return 0;
 }
@@ -475,13 +541,13 @@ int cn_gst_finalize(cn_gst* g) {
 int cn_gst_reset(cn_gst* g, void* stream) {
   if (!g) return cn_set_error("cn_gst_reset: null argument");
   cudaSetDevice(g->device);
-  const size_t n = (size_t)GST_T * g->N * g->H;
-  std::vector<float> inv(n * 2, GST_INVALID);
+  const size_t n = (size_t)GT_T * g->N * g->H;
+  std::vector<float> inv(n * 2, GT_INVALID);
   cudaError_t err = cudaMemcpyAsync(g->ring_pos, inv.data(), n * 2 * sizeof(float), cudaMemcpyHostToDevice, (cudaStream_t)stream);
   if (err == cudaSuccess) err = cudaStreamSynchronize((cudaStream_t)stream);
   if (err == cudaSuccess) err = cudaMemsetAsync(g->ring_mask, 0, n, (cudaStream_t)stream);
   if (err != cudaSuccess) return cn_set_error("cn_gst_reset: %s", cudaGetErrorString(err));
-  g->newest = GST_T - 1;
+  g->newest = GT_T - 1;
   return 0;
 }
 
@@ -494,29 +560,57 @@ int cn_gst_step(cn_gst* g, const float* d_robot_node, const float* d_spatial2, c
   if (!g || !d_robot_node || !d_spatial2 || !d_visible || !d_spatial_out) return cn_set_error("cn_gst_step: null argument");
   if (!g->finalized) return cn_set_error("cn_gst_step: call cn_gst_finalize after setting the parameters");
   CnDeviceGuard guard(g->device);
-  g->newest = (g->newest + 1) % GST_T;
-  if (g->tc) {
-    g->launches += 1;
-    if (g->compact)
-      return cn_gst_tcc_step(g->tc, g->ring_pos, g->ring_mask, g->newest, d_robot_node, d_spatial2, d_visible, d_reward, d_penalty,
-                             d_spatial_out, (cudaStream_t)stream);
-    return cn_gst_tc_step(g->tc, g->ring_pos, g->ring_mask, g->newest, d_robot_node, d_spatial2, d_visible, d_reward, d_penalty,
-                          d_spatial_out, (cudaStream_t)stream);
+  g->newest = (g->newest + 1) % GT_T;
+  CnLaunchCtx* p = &g->ctx;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int N = g->N, H = g->H;
+  const int R = N * GT_T * H, Rd = N * H, G = N * GT_T;
+  const int* cntR = g->counts;          // valid observation rows
+  const int* cntD = g->counts + 1;      // humans visible in the newest frame
+  const dim3 rows_grid((unsigned)(p->num_sms * 4)), grp_grid((unsigned)((G + GTC_WARPS - 1) / GTC_WARPS));
+  auto encoder = [&](int maxrows, const int* cnt, int groups, const int* start) {
+    gemm_tc(p, st, g->tX, g->tWin, maxrows, 192, 64, 64, g->w.bin, CN_ACT_NONE, out32(g->QKV, 192), cnt);
+    launch_k(p, gtc_attn_kernel, dim3((unsigned)groups), dim3((unsigned)(8 * H)), 0, st, H, start, g->QKV, g->w.bin + 64, g->tA.hi, g->tA.lo);
+    gemm_tc(p, st, g->tA, g->tWout, maxrows, 64, 64, 64, g->w.bout, CN_ACT_NONE, out32(g->O, 64), cnt);
+    launch_k(p, gtc_res_ln_kernel, rows_grid, dim3(256), 0, st, g->w, cnt, g->X0, g->O, g->X1, g->tY.hi, g->tY.lo);
+    gemm_tc(p, st, g->tY, g->tW1, maxrows, 128, 64, 64, g->w.b1, CN_ACT_RELU, out16(g->tF), cnt);
+    gemm_tc(p, st, g->tF, g->tW2, maxrows, 64, 128, 64, g->w.b2, CN_ACT_NONE, out32(g->O, 64), cnt);
+    launch_k(p, gtc_res_kernel, rows_grid, dim3(256), 0, st, cnt, g->X1, g->O, g->tXS.hi, g->tXS.lo);
+    gemm_tc(p, st, g->tXS, g->tWih, maxrows, 256, 64, 256, g->w.bih, CN_ACT_NONE,
+            out32(g->GX, 256, maxrows == R ? &g->GX_R : &g->GX_Rd), cnt);
+  };
+  launch_k(p, gtc_prep_kernel, grp_grid, dim3(GTC_WARPS * 32), 0, st, N, H, g->ring_pos, g->ring_mask, g->newest, d_robot_node, d_spatial2,
+           d_visible, g->rowm, g->inp, g->gcount, g->ecount, g->fp, g->pos_last);
+  launch_k(p, gtc_scan_kernel, dim3(1), dim3(1024), 0, st, g->gcount, G, g->gstart, g->ecount, N, g->estart, g->counts);
+  launch_k(p, gtc_index_kernel, grp_grid, dim3(GTC_WARPS * 32), 0, st, N, H, g->rowm, g->fp, g->gstart, g->estart, g->cidx, g->crow,
+           g->drow);
+  launch_k(p, gtc_embed_kernel, rows_grid, dim3(256), 0, st, g->w, cntR, g->crow, g->inp, g->X0, g->tX.hi, g->tX.lo);
+  encoder(R, cntR, G, g->gstart);
+  // LSTM over the 5 observed frames, humans visible now only (h0 = c0 = 0: frame 0 has no recurrent GEMM, its
+  // hidden-state gate term is b_hh)
+  for (int t = 0; t < GT_T; ++t) {
+    if (t > 0) gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
+    launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, t, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
+             g->c32, g->tHd.hi, g->tHd.lo);
   }
-  GstW w;
-  w.We_t = g->dev[0]; w.be = g->dev[1]; w.ln0_g = g->dev[2]; w.ln0_b = g->dev[3]; w.Win_t = g->dev[4]; w.bin = g->dev[5];
-  w.Wout_t = g->dev[6]; w.bout = g->dev[7]; w.ln1_g = g->dev[8]; w.ln1_b = g->dev[9]; w.W1_t = g->dev[10]; w.b1 = g->dev[11];
-  w.W2_t = g->dev[12]; w.b2 = g->dev[13]; w.Wih_t = g->dev[14]; w.bih = g->dev[15]; w.Whh_t = g->dev[16]; w.bhh = g->dev[17];
-  w.Wp = g->dev[18]; w.bp = g->dev[19];
-  cn_pretext_kernel<<<g->N, GST_THREADS, g->smem, (cudaStream_t)stream>>>(w, g->N, g->H, g->P, g->thr, g->collision_penalty,
-                                                                           g->ring_pos, g->ring_mask, g->newest, d_robot_node,
-                                                                           d_spatial2, d_visible, d_reward, d_penalty, d_spatial_out);
-  g->launches += 1;
+  for (int tt = 0; tt < GT_T; ++tt) {
+    if (tt > 0) {
+      launch_k(p, gtc_embed_kernel, rows_grid, dim3(256), 0, st, g->w, cntD, (const int*)nullptr, g->xin, g->X0, g->tX.hi, g->tX.lo);
+      encoder(Rd, cntD, N, g->estart);
+      gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
+      launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, -1, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
+               g->c32, g->tHd.hi, g->tHd.lo);
+    }
+    launch_k(p, gtc_h2p_kernel, rows_grid, dim3(256), 0, st, g->w, tt, cntD, g->drow, g->h32, g->pos_last, g->xin, g->mu_cum, g->pred);
+  }
+  launch_k(p, gt_final_kernel, dim3((unsigned)N), dim3(32), 0, st, N, H, g->P, g->thr, g->collision_penalty, d_robot_node, d_spatial2,
+           g->fp, g->pred, d_reward, d_penalty, d_spatial_out);
   cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return cn_set_error("cn_pretext_kernel launch: %s", cudaGetErrorString(err));
+  if (err != cudaSuccess) return cn_set_error("cn_gst_step: %s", cudaGetErrorString(err));
+  if (p->launch_error) { p->launch_error = false; return 1; }
   return 0;
 }
 
-int64_t cn_gst_launch_count(cn_gst* g) { return !g ? 0 : (g->tc ? cn_gst_tc_launches(g->tc) : g->launches); }
+int64_t cn_gst_launch_count(cn_gst* g) { return g ? g->ctx.launches : 0; }
 
 }  // extern "C"

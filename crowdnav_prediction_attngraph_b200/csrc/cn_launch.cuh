@@ -4,7 +4,6 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
@@ -36,7 +35,6 @@ struct CnLaunchCtx {
   int num_sms = 132;
   bool pdl = false;             // programmatic dependent launch along the kernel chain (CN_PDL=0 disables)
   int64_t launches = 0;
-  long dbg_launch_idx = 0;      // launch index within the current step (CN_PDL_WINDOW debugging)
   bool launch_error = false;    // a launch or a GEMM output map failed (cn_last_error has the stage and the reason)
   const char* cur_stage = nullptr;   // stage name of the launches being enqueued (error reports)
   std::vector<void*> allocs;
@@ -76,15 +74,7 @@ void launch_k(CnLaunchCtx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, siz
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  // debug aid: CN_PDL_WINDOW=lo:hi keeps the attribute only for launches lo <= index < hi of the context
-  static int win_lo = -1, win_hi = -1;
-  if (win_lo < 0) {
-    const char* w = getenv("CN_PDL_WINDOW");
-    win_lo = 0; win_hi = 1 << 30;
-    if (w) sscanf(w, "%d:%d", &win_lo, &win_hi);
-  }
-  const long idx = c->dbg_launch_idx++;
-  cfg.attrs = at; cfg.numAttrs = (c->pdl && idx >= win_lo && idx < win_hi) ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = c->pdl ? 1 : 0;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
   if (e != cudaSuccess && !c->launch_error) {     // keep the FIRST failure and the stage it happened in
     c->launch_error = true;

@@ -441,7 +441,7 @@ class CudaPretextVecEnv(object):
     """`VecPretextNormalize(ShmemVecEnv([CrowdSimPredRealGST-v0 ...]))` on one GPU (BASELINE config 3, SURVEY row a16).
 
     The environments run in the engine's CrowdSimVarNum-v0 mode without sorting (that IS the raw RealGST
-    observation, crowd_sim_pred_real_gst.py:73-88); one fused kernel per step keeps the wrapper's 5-frame
+    observation, crowd_sim_pred_real_gst.py:73-88); one chain of kernels per step keeps the wrapper's 5-frame
     trajectory / mask buffers, runs the GST predictor, adds the future-collision penalty to the reward, writes the
     predicted relative positions into the 2(P+1)-wide spatial_edges and sorts the rows by distance
     (rl/vec_env/vec_pretext_normalize.py:112-191).  Like the reference, the buffers are NOT cleared when a

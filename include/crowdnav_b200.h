@@ -109,7 +109,7 @@ int cn_copy_segments(const cn_copy_seg *segs, int n, int device, void *stream);
  * read of every worker) -- ONE device->pinned-host copy of the packed step outputs on `stream`, then a wait for the stream. */
 int cn_fetch_sync(void *h_dst, const void *d_src, size_t bytes, int device, void *stream);
 
-/* BASELINE config 3: GST trajectory predictor + VecPretextNormalize processing (one fused launch per step).
+/* BASELINE config 3: GST trajectory predictor + VecPretextNormalize processing (one chain of launches per step).
  * replaces: VecPretextNormalize.reset / process_obs_rew (rl/vec_env/vec_pretext_normalize.py:85-191) and
  * CrowdNavPredInterfaceMultiEnv.forward (gst_updated/scripts/wrapper/crowd_nav_interface_parallel.py:45-114).     */
 typedef struct cn_gst cn_gst;

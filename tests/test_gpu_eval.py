@@ -121,5 +121,6 @@ def test_shipped_non_rand_checkpoint_reproduces_its_test_log_exactly():
     assert out["timeout_cases"] == [49, 299]
     assert round(out["avg_nav_time"], 2) == 15.42 and round(out["path_length"], 2) == 20.96
     # every episode outcome above is exact; the intrusion ratio counts single frames, where the 1e-6 summation-order
-    # difference of the compact predictor path moves one or two frames (4.237 vs the log's 4.23; CN_GST_MODE=tc gives 4.23)
+    # difference of the predictor's compact rows (masked neighbours enter the soft-max as one term) moves one or two
+    # frames (4.237 vs the log's 4.23)
     assert abs(out["intrusion_ratio"] - 4.23) < 0.015 and round(out["min_intrusion_dist"], 2) == 0.44

@@ -1,4 +1,4 @@
-"""GPU: BASELINE config 3 (row a16) -- the fused GST predictor + VecPretextNormalize kernel against vectors recorded
+"""GPU: BASELINE config 3 (row a16) -- the GST predictor + VecPretextNormalize step (cn_gst_step) against vectors recorded
 from the unmodified reference (tools/make_golden_gst.py) and against the oracle in lock-step."""
 import ctypes as C
 import os
@@ -50,13 +50,6 @@ def _unsort(sp2, rows):
         order = np.argsort(key[n], kind="stable")
         out[n, order] = rows[n]
     return out
-
-
-@pytest.fixture(params=["tcc", "tc", "fused"], autouse=True)
-def gst_mode(request, monkeypatch):
-    """all three implementations: compact-row tensor-core GEMMs (default), dense-row tensor-core GEMMs, single fused CUDA-core kernel"""
-    monkeypatch.setenv("CN_GST_MODE", request.param)
-    return request.param
 
 
 def test_gst_kernel_matches_reference_predictor():
