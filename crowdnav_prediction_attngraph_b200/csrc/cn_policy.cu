@@ -35,8 +35,8 @@ struct cn_policy {
   float* bqkvH = nullptr;
   int* tile_tab = nullptr;   // row tiles of the fused kernel (cn_qkv_tiles_kernel)
   cudaEvent_t ev_tiles;
-  // human-human attention instance: R queries of an environment per warp (CN_ATTN_R = 1 (default), 2 or 4; sharing
-  // K / V rows between queries does not pay, the kernel is bound by load latency at ~4 keys per query, not by L1 delivery)
+  // human-human attention instance: R queries of an environment per warp (CN_ATTN_R = 1 (default), 2 or 4; R = 1 is
+  // the fastest at H = 20, R = 2 at H = 50 and 100, DESIGN.md 3.4c)
   void (*attn_kernel)(const float*, const int*, const int*, const int*, const int*, float*, __half*, __half*);
   int attn_warps;
   int qkv_chunks;     // 1 (default): single pass; 2 (CN_QKV_CHUNKS=2): QKV + attention in two row chunks with overlap
@@ -440,8 +440,9 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   mark(p, st, 3);
   if (tcm) {
     // Optional experiment (CN_QKV_CHUNKS=2): QKV projection + attention in two row chunks split at an environment
-    // boundary so that chunk 0's attention (side stream) overlaps chunk 1's GEMM.  Off by default: the attention is
-    // load-latency bound, not L2-capacity bound, so the overlap did not pay.
+    // boundary so that chunk 0's attention (side stream) overlaps chunk 1's GEMM.  Off by default: at H = 20 the
+    // attention is load-latency bound, not L2-capacity bound, and the overlap does not pay; at H = 50 and 100 it
+    // saves 0.4-3 % of the forward (DESIGN.md 3.4c).
     const int* mid = p->row_start + N / 2;
     __half* ah = p->tAo.hi;
     __half* al = p->tAo.lo;

@@ -319,9 +319,10 @@ __global__ void __launch_bounds__(256) cn_embed1_kernel(const float* __restrict_
 //    P V): one exp per (key, head) and no rescaling of the accumulators;
 //  * the p of the other three chunks come from the neighbouring lanes of the aligned 4-lane group.
 //  * template parameter R: R query rows of the SAME environment share every K / V row a warp loads (each loaded
-//    element then feeds R FMAs).  R = 1 was the fastest of the three when measured at 4096 envs -- the
-//    L1 delivery rate (one FMA per 4 bytes) is not what limits the kernel, the extra registers cost occupancy; R = 1
-//    is the default, the others stay selectable with CN_ATTN_R for other crowd sizes.
+//    element then feeds R FMAs).  At 4096 envs and H = 20 (about 4 keys per query) R = 1 is the fastest of the
+//    three -- the L1 delivery rate (one FMA per 4 bytes) is not what limits the kernel, the extra registers cost
+//    occupancy.  At H = 50 and 100 R = 2 is faster (0.219 against 0.232-0.235 ms, 0.663 against 0.772-0.776 ms;
+//    DESIGN.md §3.4c).  R = 1 is the default; CN_ATTN_R selects the others.
 #define CN_ATTN_WARPS 4
 #define CN_ATTN_MAXKEYS 128
 template <int R, int KB /* keys whose rows are in flight together */, int W /* warps per CTA */>
