@@ -53,6 +53,7 @@ struct CnParams {
   double sf_A, sf_B, sf_KI;   // config.sf
   int defer_tries;        // warp-scope rejection-sampling budget (cn_env_event_kernel -> cn_env_event_heavy_kernel)
   int robot_policy;       // robot.policy: 0 caller's action, 1 'orca', 2 'social_force' (cn_robot_act)
+  int robot_visible;      // robot.visible: the humans' solves take the robot as one more agent (cn_orca_build, cn_sf_action)
 };
 
 // Struct-of-arrays environment state in HBM.  Per-human arrays are [N][H] (human index
@@ -89,7 +90,7 @@ struct CnState {
   uint8_t *vis;                      // human_visibility (to the robot)
   // per-human cached rvo2 simulator parameters (crowd_nav/policy/orca.py:79-95): frozen at creation
   uint8_t *sim_exists;               // [N][H]
-  uint8_t *sim_n;                    // [N][H] live human count when the simulator was created (human_num_range > 0)
+  uint8_t *sim_n;                    // [N][H] agent count when the simulator was created (human_num_range > 0 or robot visible)
   float *sim_nd, *sim_rself, *sim_vmax;   // [N][H]
   float *sim_rother;                 // [N][H][H] (only when randomize)
   // legacy numpy MT19937 per environment

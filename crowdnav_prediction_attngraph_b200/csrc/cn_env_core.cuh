@@ -32,6 +32,15 @@
 #define CN_HEAVY_THREADS 512
 #define CN_DEFER_TRIES 136
 
+// robot.visible code paths (cn_orca_build, cn_sf_action) exist only in the step kernel's VIS instantiations, so the
+// network policy's kernels without a visible robot carry none of them.  The host build of this header (the test
+// harness) keeps them all and lets CnParams::robot_visible decide at run time.
+#if defined(__CUDA_ARCH__)
+#define CN_VIS(VIS) (VIS)
+#else
+#define CN_VIS(VIS) true
+#endif
+
 CN_HD double cn_fma(double a, double b, double c) {
 #if defined(__CUDA_ARCH__)
   return __fma_rn(a, b, c);
@@ -218,7 +227,11 @@ CN_HD void cn_phase_load(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
 // `mark`: value written to sim_exists for a simulator this call creates: 1, or 2 = PROVISIONAL when the solve runs ahead of
 // the step it belongs to (pre-solve on the side stream, cn_env_kernels.cu): the finishing pass of that step promotes 2 / 3 -> 1;
 // a full solve treats anything but 1 as missing, so an abandoned pre-solve (state uploaded in between) leaves no trace.
-template <int MAXH>
+// VIS (robot.visible, crowd_sim.py:695-699): get_human_actions (use_fov) appends the robot -- or, outside the human's FOV,
+// the dummy robot at (7, 7) with velocity 0 -- as the simulator's last agent, index hn; its radius is robot.radius either
+// way.  The ground-truth look-ahead (use_fov = false) shows the humans only, so in phase 'test' the agent count alternates
+// between hn + 1 and hn and every count change re-creates the simulator (orca.py:80-89).
+template <int MAXH, bool VIS = false>
 CN_HD void cn_orca_build(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h, CnLineStore lines, int& nl_out,
                          float& vmax_out, CnF2& pref_out, bool use_fov = true, uint8_t mark = 1) {
   const int H = p.H;            // slots (row pitch of the [N][H] arrays)
@@ -227,18 +240,22 @@ CN_HD void cn_orca_build(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
   const double fov = p.human_fov;
   float nd, rself, vmax;
   const double pad = 0.01;
+  const bool with_robot = CN_VIS(VIS) && p.robot_visible && use_fov;
   // --- cached simulator parameters (frozen at creation; orca.py:80-95 only updates pos/vel)
   if (p.randomize) {
-    // (re)created when missing or when humans joined / left since its creation (orca.py:80-82: agent count mismatch)
+    // (re)created when missing or when the agent count changed since its creation (orca.py:80-82): humans joined /
+    // left, or (robot visible) the robot joined / left between get_human_actions and the look-ahead
     const uint8_t ex = g.sim_exists[i];
-    if (ex != 1 || (p.hrange > 0 && g.sim_n[i] != (uint8_t)hn)) {
-      g.sim_n[i] = (uint8_t)hn;
+    const uint8_t count = (uint8_t)(hn + (with_robot ? 1 : 0));
+    if (ex != 1 || ((p.hrange > 0 || CN_VIS(VIS)) && g.sim_n[i] != count)) {
+      g.sim_n[i] = count;
       g.sim_nd[i] = (float)g.nd_global[e];
       g.sim_rself[i] = (float)(s.rad[h] + pad + p.orca_safety_space);
       g.sim_vmax[i] = (float)s.vpref[h];
       for (int j = 0; j < hn; ++j) {
         if (j == h) continue;
-        const bool v = cn_in_fov(s.px[h], s.py[h], s.vx[h], s.vy[h], s.px[j], s.py[j], fov);
+        // a simulator the look-ahead creates takes every human as is (no FOV dummies)
+        const bool v = (CN_VIS(VIS) && !use_fov) || cn_in_fov(s.px[h], s.py[h], s.vx[h], s.vy[h], s.px[j], s.py[j], fov);
         g.sim_rother[i * H + j] = (float)((v ? s.rad[j] : 0.3) + pad + p.orca_safety_space);
       }
       // a pre-solve that RE-creates an official simulator (human count changed) marks it 3: still "exists" to a reader
@@ -278,9 +295,25 @@ CN_HD void cn_orca_build(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
     const float d = f2abssq(f2sub(pos, op));
     if (d < rangeSq) { vd[nl] = d; vj[nl] = (uint8_t)(j | (v ? 0 : 0x80)); ++nl; }
   }
+  // the robot (VIS) is kept out of vd / vj: it is the last agent, so it ranks behind every human at an equal distance
+  float rd = 0.0f;
+  bool rin = false;
+  if (with_robot) {
+    const bool v = cn_in_fov(s.px[h], s.py[h], s.vx[h], s.vy[h], s.rpx, s.rpy, fov);
+    const CnF2 op = v ? f2((float)s.rpx, (float)s.rpy) : f2(7.0f, 7.0f);        // dummy_robot (crowd_sim.py:135-139)
+    const CnF2 ov = v ? f2(s.rvx, s.rvy) : f2(0.0f, 0.0f);
+    rd = f2abssq(f2sub(pos, op));
+    rin = rd < rangeSq;
+    if (rin) {
+      int rank = 0;
+      for (int b = 0; b < nl; ++b) rank += (vd[b] <= rd) ? 1 : 0;
+      lines.set(rank, cn_orca_line(pos, vel, rself, op, ov, (float)(p.robot_radius + pad + p.orca_safety_space),
+                                   invTimeHorizon, timeStep));
+    }
+  }
   for (int a = 0; a < nl; ++a) {
     const float da = vd[a];
-    int rank = 0;
+    int rank = (rin && rd < da) ? 1 : 0;
     for (int b = 0; b < nl; ++b) rank += (vd[b] < da || (vd[b] == da && b < a)) ? 1 : 0;
     const int j = vj[a] & 0x7f;
     const bool dummy = (vj[a] & 0x80) != 0;
@@ -290,13 +323,16 @@ CN_HD void cn_orca_build(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
                                    : (float)((dummy ? 0.3 : s.rad[j]) + pad + p.orca_safety_space);
     lines.set(rank, cn_orca_line(pos, vel, rself, op, ov, orad, invTimeHorizon, timeStep));
   }
-  nl_out = nl; vmax_out = vmax; pref_out = pref;
+  nl_out = nl + (rin ? 1 : 0); vmax_out = vmax; pref_out = pref;
 }
 
 // Social-force humans (humans.policy = 'social_force', crowd_nav/policy/social_force.py:11-49): pull towards the goal
 // with relaxation K_I, exponential push A exp((r_i + r_j - d) / B) from every other human (the ones outside the FOV are
 // replaced by the dummy at (7, 7), crowd_sim.py:680-703), explicit Euler step, speed clipped to v_pref.  fp64 like the
 // reference's Python floats, same expression order.  Writes s.nwx / s.nwy and the robot-collision distance.
+// VIS (robot.visible): the robot, or outside the FOV the dummy robot at (7, 7), pushes too, radius robot.radius; it is
+// the last term of the sum.
+template <bool VIS = false>
 CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h, bool use_fov = true) {
   const int hn = s.hn;
   const double px = s.px[h], py = s.py[h], vx = s.wx[h], vy = s.wy[h];
@@ -312,6 +348,14 @@ CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, 
     const double ex = px - ox, ey = py - oy;
     const double d = sqrt(ex * ex + ey * ey);
     const double w = p.sf_A * exp((s.rad[h] + orad - d) / p.sf_B);
+    ivx += w * (ex / d);
+    ivy += w * (ey / d);
+  }
+  if (CN_VIS(VIS) && p.robot_visible && use_fov) {
+    const bool v = cn_in_fov(px, py, vx, vy, s.rpx, s.rpy, p.human_fov);
+    const double ex = px - (v ? s.rpx : 7.0), ey = py - (v ? s.rpy : 7.0);
+    const double d = sqrt(ex * ex + ey * ey);
+    const double w = p.sf_A * exp((s.rad[h] + p.robot_radius - d) / p.sf_B);
     ivx += w * (ex / d);
     ivy += w * (ey / d);
   }

@@ -68,8 +68,8 @@ __device__ inline CnEnvSh* env_view(unsigned char* base, const EnvSmemLayout& L,
 // (g.prep_*, computed off the critical path by cn_env_event_kernel) and emit its first observation in
 // the same launch.  mode 1 = reset of the whole vector env: no step, every environment installs.
 // ROBOT: robot_policy != 0 (the robot's ORCA / social-force solve, cn_robot_act); a separate instantiation so the network
-// policy's kernel carries none of its code.
-template <int MAXH, int MAXW, bool ROBOT>
+// policy's kernel carries none of its code.  VIS: robot_visible != 0 (the humans' solves see the robot), likewise.
+template <int MAXH, int MAXW, bool ROBOT, bool VIS>
 __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState g, const float* __restrict__ action,
                                                           CnObs ob, CnStepOut out, int epb, int line_cap, int mode) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
     float vmax = 0.0f;
     CnF2 pref = f2(0.0f, 0.0f);
     result = f2(0.0f, 0.0f);
-    if (live) cn_orca_build<MAXH>(p, g, *s, e, h, W.of(lane), nl, vmax, pref, use_fov, mode == 3 ? (uint8_t)2 : (uint8_t)1);
+    if (live) cn_orca_build<MAXH, VIS>(p, g, *s, e, h, W.of(lane), nl, vmax, pref, use_fov, mode == 3 ? (uint8_t)2 : (uint8_t)1);
     __syncwarp();
     cn_orca_lp2_warp(hco, W, nl, vmax, pref, result, fail);           // per half-warp; idle lanes with nl = 0
     if (fail >= 0) {
@@ -167,10 +167,10 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
     if (threadIdx.x == 0) { *lp3_count = 0; *lp3_head = 0; }          // ready for the next solve (a barrier follows)
   };
   if (mode != 1 && p.social_force) {
-    if (live) cn_sf_action(p, g, *s, e, h);                           // social-force humans: no linear programs
+    if (live) cn_sf_action<VIS>(p, g, *s, e, h);                           // social-force humans: no linear programs
   } else if (mode == 2) {
-    // finishing pass of a step whose ORCA solve already ran on the side stream (mode 3, same state: the humans do not
-    // see the robot, so their solve does not depend on this step's action)
+    // finishing pass of a step whose ORCA solve already ran on the side stream (mode 3, same state: the humans' solve
+    // reads the robot's position and velocity as the previous step left them, never this step's action)
     if (live) {
       const size_t i = cn_idx(p, e, h);
       const int nlf = g.pre_nlf[i];
@@ -464,15 +464,20 @@ int dev_alloc(cn_env* env, const char* name, T** ptr, size_t count) {
 
 typedef void (*KernelFn)(CnParams, CnState, const float*, CnObs, CnStepOut, int, int, int);
 
-KernelFn pick_kernel(int maxh, bool robot) {
+template <bool VIS>
+KernelFn pick_kernel_vis(int maxh, bool robot) {
   if (robot) {
-    if (maxh <= 32) return cn_env_step_kernel<32, 16, true>;
-    if (maxh <= 64) return cn_env_step_kernel<64, 16, true>;
-    return cn_env_step_kernel<128, 16, true>;
+    if (maxh <= 32) return cn_env_step_kernel<32, 16, true, VIS>;
+    if (maxh <= 64) return cn_env_step_kernel<64, 16, true, VIS>;
+    return cn_env_step_kernel<128, 16, true, VIS>;
   }
-  if (maxh <= 32) return cn_env_step_kernel<32, 16, false>;
-  if (maxh <= 64) return cn_env_step_kernel<64, 16, false>;
-  return cn_env_step_kernel<128, 16, false>;
+  if (maxh <= 32) return cn_env_step_kernel<32, 16, false, VIS>;
+  if (maxh <= 64) return cn_env_step_kernel<64, 16, false, VIS>;
+  return cn_env_step_kernel<128, 16, false, VIS>;
+}
+
+KernelFn pick_kernel(int maxh, bool robot, bool vis) {
+  return vis ? pick_kernel_vis<true>(maxh, robot) : pick_kernel_vis<false>(maxh, robot);
 }
 
 CnObs to_obs(const cn_obs_ptrs* o) {
@@ -525,7 +530,7 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
     env->prep_dirty = false;
   }
   const int grid = (env->p.N + env->epb - 1) / env->epb;
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0);
   // mode 0 with a pre-solve of this state done on the side stream (joined above) -> finishing pass only (mode 2)
   const int kmode = (mode == 0 && env->presolved) ? 2 : mode;
   env->presolved = false;
@@ -549,10 +554,11 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
   }
   if (env->profile) cudaEventRecord(env->pev[3], env->side);
   if (env->presolve) {
-    // PRE-SOLVE: the humans never see the robot (robot.visible = False is the only supported setting), so their ORCA
-    // solve of the NEXT step depends on the state this step leaves behind (after the event kernel's goal changes and
-    // the installed episodes) and on nothing the policy is about to compute.  It runs here, on the side stream, while
-    // the caller's stream runs the policy; the next step only finishes (robot move, reward, integration, observation).
+    // PRE-SOLVE: the humans' ORCA solve of the NEXT step depends on the state this step leaves behind (after the event
+    // kernel's goal changes and the installed episodes) and on nothing the policy is about to compute.  With the robot
+    // visible it also reads the robot's position and velocity, and both are final once this step has integrated (the
+    // next action moves the robot only after the humans' solve).  It runs here, on the side stream, while the caller's
+    // stream runs the policy; the next step only finishes (robot move, reward, integration, observation).
     fn<<<grid, env->threads, env->smem_bytes, env->side>>>(env->p, env->g, nullptr, to_obs(o), out, env->epb, env->line_cap, 3);
     env->launches += 1;
     err = cudaGetLastError();
@@ -657,6 +663,16 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
     return cn_set_error("cn_env_create: the ORCA / social-force robot is covered for CrowdSimVarNum-v0 (const_vel 0) with "
                         "human_num_range 0");
   }
+  if (cfg->robot_visible != 0 && cfg->robot_visible != 1) {
+    cn_env_destroy(env);
+    return cn_set_error("cn_env_create: robot_visible %d unsupported (0 or 1)", cfg->robot_visible);
+  }
+  if (cfg->robot_visible && cfg->const_vel) {
+    cn_env_destroy(env);
+    return cn_set_error("cn_env_create: robot_visible is covered for CrowdSimVarNum-v0 (const_vel 0) only: the reference's "
+                        "CrowdSimPred-v0 cannot run it (calc_human_future_traj('const_vel') assigns the humans' (H, 2) "
+                        "velocities into an (H + 1, 2) slice and raises on the first reset)");
+  }
   if (cfg->phase != 0 && cfg->phase != 2) {
     cn_env_destroy(env);
     return cn_set_error("cn_env_create: phase %d unsupported (0 = 'train', 2 = 'test')", cfg->phase);
@@ -674,6 +690,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   p.social_force = cfg->human_policy == 1 ? 1 : 0;
   p.sf_A = cfg->sf_A; p.sf_B = cfg->sf_B; p.sf_KI = cfg->sf_KI;
   p.robot_policy = cfg->robot_policy;
+  p.robot_visible = cfg->robot_visible;
   {
     // warp-scope budget of rejection-sampling tries before an event goes to the CTA-scope kernel
     // (CN_DEFER_TRIES=1 sends every search that needs a second candidate there: parity tests of the heavy path)
@@ -741,10 +758,12 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   const EnvSmemLayout L = env_layout(p.H, true, p.social_force != 0);
   int nsm = 0;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0);
   err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
   if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(err)); }
-  const int cap_max = p.H > 1 ? p.H - 1 : 1;
+  // ORCA lines per human: one per other human, plus one for the robot when it is visible
+  const int max_lines = p.H - 1 + p.robot_visible;
+  const int cap_max = max_lines > 1 ? max_lines : 1;
   int best_epb = 0, best_cap = 0, best_threads = 0;
   size_t best_need = 0;
   bool best_single = false;
@@ -776,7 +795,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   {
     // global scratch for the overflow lines (k >= line_cap) of every step-kernel thread
     float4* ovf = nullptr;
-    env->g.ovf_stride = (p.H - 1 - env->line_cap) > 0 ? (p.H - 1 - env->line_cap) : 1;
+    env->g.ovf_stride = (max_lines - env->line_cap) > 0 ? (max_lines - env->line_cap) : 1;
     int rc2 = dev_alloc(env, nullptr, &ovf, (size_t)grid * env->threads * env->g.ovf_stride);
     if (rc2) { cn_env_destroy(env); return rc2; }
     env->g.line_ovf = ovf;

@@ -93,8 +93,8 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         phase = "test" if (nenv_total or num_envs) == 1 else "train"
     if phase not in ("train", "test"):
         raise NotImplementedError("phase %r: the engine covers 'train' and 'test'" % (phase,))
-    if config.action_space.kinematics != "holonomic" or config.robot.visible:
-        raise NotImplementedError("engine covers the holonomic robot with robot.visible=False")
+    if config.action_space.kinematics != "holonomic":
+        raise NotImplementedError("engine covers the holonomic robot")
     if config.humans.policy not in ("orca", "social_force"):
         raise NotImplementedError("humans.policy %r: the engine covers 'orca' and 'social_force'" % (config.humans.policy,))
     if env_name == "CrowdSimPred-v0":
@@ -105,6 +105,12 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         const_vel = 0
     else:
         raise NotImplementedError("env id %r is not covered by the CUDA engine" % env_name)
+    robot_visible = bool(config.robot.visible)
+    if robot_visible and const_vel:
+        raise NotImplementedError(
+            "robot.visible=True on CrowdSimPred-v0 is not covered: the reference cannot run it (calc_human_future_traj("
+            "'const_vel') assigns prev_human_pos[:, 2:4], shape (H, 2), into an (H + 1, 2) slice, crowd_sim_var_num.py:"
+            "155,174, and raises on the first reset)")
     # robot.policy 'orca' / 'social_force': the robot is driven inside env.step and the caller's action is ignored
     # (crowd_sim_var_num.py:371-377); any other name (a network policy) takes the caller's action
     robot_policy = ROBOT_POLICIES.get(getattr(config.robot, "policy", None), 0)
@@ -141,6 +147,7 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         orca_neighbor_dist=float(config.orca.neighbor_dist), orca_safety_space=float(config.orca.safety_space),
         orca_time_horizon=float(config.orca.time_horizon),
         human_policy=1 if config.humans.policy == "social_force" else 0, robot_policy=robot_policy,
+        robot_visible=int(robot_visible),
         sf_A=float(config.sf.A), sf_B=float(config.sf.B), sf_KI=float(config.sf.KI),
         phase=2 if phase == "test" else 0, val_size=int(getattr(config.env, "val_size", 100)),
         test_size=int(getattr(config.env, "test_size", 500)))

@@ -60,9 +60,14 @@ typedef struct cn_config {
   int32_t human_num_range;        /* sim.human_num_range: humans join / leave every 5 s; observations are padded to
                                    * human_num + human_num_range rows (crowd_sim_pred.py:165-194)             */
   int32_t human_policy;           /* humans.policy: 0 'orca', 1 'social_force' (crowd_nav/policy/social_force.py) */
-  int32_t robot_policy;           /* robot.policy: 0 the caller's action (a network policy), 1 'orca', 2 'social_force':
+  int16_t robot_policy;           /* robot.policy: 0 the caller's action (a network policy), 1 'orca', 2 'social_force':
                                    * the step computes the robot's velocity itself and ignores d_action
                                    * (crowd_sim_var_num.py:371-377); CrowdSimVarNum-v0 with human_num_range 0 only */
+  int16_t robot_visible;          /* robot.visible: 1 = every human's ORCA / social-force solve sees the robot (or, outside
+                                   * the human's FOV, the dummy robot at (7, 7)) as one more agent (crowd_sim.py:695-699);
+                                   * CrowdSimVarNum-v0 only.  robot_policy and robot_visible share the 4 bytes robot_policy
+                                   * had as an int32, so the struct keeps its size and every offset (little-endian: a caller
+                                   * that stores robot_policy as an int32 below 32768 leaves robot_visible 0)          */
   double time_step, time_limit, pred_timestep;
   double circle_radius, arena_size;
   double discomfort_dist, discomfort_penalty_factor, success_reward, collision_penalty;

@@ -72,6 +72,28 @@ CASES = {
     "env_varnum_h10_sf_robot_rand": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
                                          robot_policy="social_force", randomize=True, goal_changing=True, nenv=2,
                                          steps=200, seed=31),
+    # robot.visible = True (crowd_sim.py:695-699): every human's ORCA / social-force solve gets the robot (or, outside
+    # the human's FOV, the dummy robot at (7, 7) with config.robot.radius) as its last agent.  The test-phase case
+    # rebuilds each simulator twice per step (hn + 1 agents in get_human_actions, hn in the look-ahead); the range
+    # case moves the robot's index with the live count; humans.FOV = 1.0 makes the dummy robot actually occur.
+    "env_varnum_h5_vis": dict(env_name="CrowdSimVarNum-v0", human_num=5, predict_method="none", robot_visible=True,
+                              randomize=False, goal_changing=False, nenv=4, steps=200, seed=425),
+    "env_varnum_h20_vis_rand": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                    robot_visible=True, randomize=True, goal_changing=True, nenv=3, steps=180, seed=425),
+    "env_varnum_h20_test_vis_rand": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                         robot_visible=True, randomize=True, goal_changing=True, nenv=2, steps=120,
+                                         seed=11, phase="test"),
+    "env_varnum_h6_range2_vis": dict(env_name="CrowdSimVarNum-v0", human_num=6, predict_method="none", human_num_range=2,
+                                     robot_visible=True, randomize=True, goal_changing=True, nenv=3, steps=200, seed=9),
+    "env_varnum_h8_sf_vis": dict(env_name="CrowdSimVarNum-v0", human_num=8, predict_method="none",
+                                 human_policy="social_force", robot_visible=True, randomize=True, goal_changing=True,
+                                 nenv=2, steps=160, seed=21),
+    "env_varnum_h10_orca_robot_vis_rand": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
+                                               robot_policy="orca", robot_visible=True, randomize=True,
+                                               goal_changing=True, nenv=2, steps=200, seed=31),
+    "env_varnum_h10_vis_fov1": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
+                                    robot_visible=True, human_fov=1.0, randomize=True, goal_changing=True, nenv=3,
+                                    steps=200, seed=17),
 }
 
 
@@ -105,6 +127,9 @@ def build_reference_env(case, rank):
     cfg.env.randomize_attributes = case["randomize"]
     cfg.humans.random_goal_changing = case["goal_changing"]
     cfg.orca.neighbor_dist = 10
+    cfg.robot.visible = case.get("robot_visible", False)
+    if "human_fov" in case:
+        cfg.humans.FOV = case["human_fov"]
     env = gym.make(case["env_name"])
     env.configure(cfg)
     env.thisSeed = case["seed"] + rank
