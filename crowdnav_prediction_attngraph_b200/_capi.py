@@ -49,6 +49,16 @@ class CnActPtrs(C.Structure):
         "value", "action", "log_prob", "h_out", "action_mean")]
 
 
+class CnDsrnnConfig(C.Structure):
+    _fields_ = [("num_envs", C.c_int32), ("human_num", C.c_int32), ("input_size", C.c_int32), ("device", C.c_int32)]
+
+
+class CnDsrnnActPtrs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in (
+        "robot_node", "temporal_edges", "spatial_edges", "h_in", "edge_h_in", "masks", "noise",
+        "value", "action", "log_prob", "h_out", "edge_h_out", "action_mean")]
+
+
 # every symbol include/crowdnav_b200.h declares (tests check the library exports all of them)
 ABI_VERSION = 3          # include/crowdnav_b200.h CN_ABI_VERSION
 
@@ -62,6 +72,8 @@ EXPORTS = [
     "cn_gst_launch_count",
     "cn_update_linear_saved_bytes", "cn_update_linear_ws_bytes", "cn_update_linear_fwd", "cn_update_linear_bwd",
     "cn_update_attn_fwd", "cn_update_attn_bwd", "cn_update_gru_fwd", "cn_update_gru_bwd",
+    "cn_dsrnn_create", "cn_dsrnn_destroy", "cn_dsrnn_set_param", "cn_dsrnn_finalize", "cn_dsrnn_act",
+    "cn_dsrnn_launch_count", "cn_dsrnn_profile", "cn_dsrnn_stage_count", "cn_dsrnn_stage_name", "cn_dsrnn_stage_ms",
 ]
 
 _lib = None
@@ -153,6 +165,18 @@ def load_library(path=None):
     lib.cn_policy_stage_name.restype = C.c_char_p
     lib.cn_policy_stage_name.argtypes = [C.c_int]
     lib.cn_policy_stage_ms.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    lib.cn_dsrnn_create.argtypes = [C.POINTER(CnDsrnnConfig), C.POINTER(C.c_void_p)]
+    lib.cn_dsrnn_destroy.argtypes = [C.c_void_p]
+    lib.cn_dsrnn_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t]
+    lib.cn_dsrnn_finalize.argtypes = [C.c_void_p, C.c_void_p]
+    lib.cn_dsrnn_act.argtypes = [C.c_void_p, C.POINTER(CnDsrnnActPtrs), C.c_void_p]
+    lib.cn_dsrnn_launch_count.restype = C.c_int64
+    lib.cn_dsrnn_launch_count.argtypes = [C.c_void_p]
+    lib.cn_dsrnn_profile.argtypes = [C.c_void_p, C.c_int]
+    lib.cn_dsrnn_stage_count.restype = C.c_int
+    lib.cn_dsrnn_stage_name.restype = C.c_char_p
+    lib.cn_dsrnn_stage_name.argtypes = [C.c_int]
+    lib.cn_dsrnn_stage_ms.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.cn_update_linear_saved_bytes.restype = C.c_size_t
     lib.cn_update_linear_saved_bytes.argtypes = [C.c_int, C.c_int]
     lib.cn_update_linear_ws_bytes.restype = C.c_size_t

@@ -136,6 +136,9 @@ int tc_set_attrs() {
     }
   if (e == cudaSuccess)
     e = cudaFuncSetAttribute(cn_gemm_tc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::kSmemBytes);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(cn_gemm_tc_kernel<256, false, CN_ACT_NONE, TC_OUT_GRU>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<256>::kSmemBytes);
   if (e != cudaSuccess) return cn_set_error("cudaFuncSetAttribute(tc): %s", cudaGetErrorString(e));
   return 0;
 }
@@ -196,6 +199,30 @@ void gemm_tc(CnLaunchCtx* c, cudaStream_t st, const TcMat& A, const TcMat& B, in
   else
     launch_k(c, tc_kernel<64>(act, out_kind), grid, dim3(TC_THREADS), TcCfg<64>::kSmemBytes, st, A.mh, A.ml, B.mh, B.ml, M, N, K, ep,
              *mc, *mh, *ml);
+}
+
+void gemm_tc_gru(CnLaunchCtx* c, cudaStream_t st, const TcMat& A, const TcMat& B, int M, const float* bias,
+                 const float* h_in, const float* mask, float* h_out, int group, int pitch, int off, __half* oh, __half* ol,
+                 int ldh) {
+  const int N = 4 * 256, K = 64 + 256;
+  if (A.box_k != tc_box_k(256) || B.box_k != tc_box_k(256) || !bias || !h_out || !mask || group <= 0) {
+    if (!c->launch_error) {
+      c->launch_error = true;
+      cn_set_error("gemm_tc_gru in stage '%s': operand boxes %d / %d wide (need %d), or a missing bias / mask / output",
+                   c->cur_stage ? c->cur_stage : "?", A.box_k, B.box_k, tc_box_k(256));
+    }
+    return;
+  }
+  TcEpilogue ep;
+  memset(&ep, 0, sizeof(ep));
+  ep.bias = bias; ep.inv_scale = 1.0f / 64.0f; ep.act_hi = 1 << 30;
+  ep.c32 = h_out; ep.ldc = 256; ep.out_hi = oh; ep.out_lo = ol; ep.ldh = ldh;
+  ep.gru_h = h_in; ep.gru_mask = mask; ep.gru_group = group; ep.gru_pitch = pitch; ep.gru_off = off;
+  static const CUtensorMap no_map = {};
+  const int tiles = (N / 256) * ((M + TC_BM - 1) / TC_BM);
+  dim3 grid(tiles < c->num_sms ? tiles : c->num_sms);
+  launch_k(c, cn_gemm_tc_kernel<256, false, CN_ACT_NONE, TC_OUT_GRU>, grid, dim3(TC_THREADS), TcCfg<256>::kSmemBytes, st,
+           A.mh, A.ml, B.mh, B.ml, M, N, K, ep, no_map, no_map, no_map);
 }
 
 int gemm_tc_promote(int num_sms, cudaStream_t st, const __half* ahi, const __half* alo, int a_rows, int a_pitch,

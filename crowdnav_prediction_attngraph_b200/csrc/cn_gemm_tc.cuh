@@ -77,6 +77,13 @@ struct TcEpilogue {
   int ksplit;                 // > 1 (PROMOTE only): the K range is cut into `ksplit` slices, every slice is its own tile and ADDS its
                               // partial product into a zero-initialised fp32 C with atomic adds (bias from slice 0
                               // only, no activation): wgrad has K = #rows (hundreds of thousands) and a tiny output
+  // --- GRU cell epilogue (TC_OUT_GRU, the DS-RNN edge GRUs); all zero / null otherwise ---
+  // GEMM row r is the state row  out_r = (r / gru_group) * gru_pitch + gru_off + r % gru_group  of the [*, 256] fp32
+  // state: h = gru_h[out_r] * gru_mask[r / gru_group] (gru_h null: h = 0); h' goes to c32[out_r] (ldc = 256) and, with
+  // out_hi, as a split fp16 pair to out_hi / out_lo [r, ldh].
+  const float* gru_h;
+  const float* gru_mask;
+  int gru_group, gru_pitch, gru_off;
 #ifdef CN_GEMM_TRACE
   unsigned long long* trace;  // [gridDim.x][trace_cap][TC_TRACE_REC] per-tile records (tools/gemm_tile_trace.py)
   int trace_cap;
@@ -91,8 +98,9 @@ struct TcEpilogue {
 #define TC_TRACE_WAIT_CLK 100     // a wait on a buffer that is already free returns well within this many cycles
 #endif
 
-// Output kinds of the non-PROMOTE instances (template parameter OUT): fp32 C, split fp16 (hi, lo), or both
-enum { TC_OUT_F32 = 1, TC_OUT_F16 = 2, TC_OUT_BOTH = 3 };
+// Output kinds of the non-PROMOTE instances (template parameter OUT): fp32 C, split fp16 (hi, lo), or both; or
+// (BN = 256 only) the GRU cell epilogue tc_epilogue_gru
+enum { TC_OUT_F32 = 1, TC_OUT_F16 = 2, TC_OUT_BOTH = 3, TC_OUT_GRU = 4 };
 
 #ifdef CN_GEMM_TRACE
 #define TC_TRACE(...) __VA_ARGS__
@@ -452,6 +460,55 @@ __device__ __forceinline__ void tc_epilogue_tma(const float (&acc)[128], const T
   }
 }
 
+// GRU cell epilogue (TC_OUT_GRU, BN = 256): the B operand is interleaved so that columns [0, 64), [64, 128),
+// [128, 192), [192, 256) of the tile at n0 hold the pre-activations r, z, gi_n = W_in x + b_in and gh_n = W_hn h + b_hn
+// of hidden units n0 / 4 .. n0 / 4 + 63.  Accumulator column group g (< 8) of this thread and the groups g + 8, + 16,
+// + 24 are then the four gates of the same two units, and the cell finishes in registers (PyTorch's GRU,
+// h' = (1 - z) n + z h with n = tanh(gi_n + r gh_n)).  No gate leaves the SM: h' is stored in fp32 straight into the
+// state row of the GEMM row (TcEpilogue::gru_*), and optionally as a split fp16 pair in GEMM row order.
+__device__ __forceinline__ float tc_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+__device__ __forceinline__ void tc_epilogue_gru(const float (&acc)[128], const TcEpilogue& ep, float inv_scale, int n0,
+                                                int r0, int cq, int m_ext) {
+  const int u0 = n0 / 4;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = r0 + 8 * h;
+    if (row >= m_ext) continue;
+    const int env = row / ep.gru_group;
+    const size_t orow = (size_t)env * ep.gru_pitch + ep.gru_off + (row - env * ep.gru_group);
+    const float m = ep.gru_h ? __ldg(ep.gru_mask + env) : 0.0f;
+#pragma unroll
+    for (int g = 0; g < 8; ++g) {
+      const int c = 8 * g + cq, u = u0 + c;
+      float hv[2] = {0.0f, 0.0f};
+      if (ep.gru_h) {
+        const float2 t = __ldg(reinterpret_cast<const float2*>(ep.gru_h + orow * 256 + u));
+        hv[0] = t.x * m; hv[1] = t.y * m;
+      }
+      float o[2];
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int a = 4 * g + 2 * h + k;
+        const float r = tc_sigmoid(fmaf(acc[a], inv_scale, __ldg(ep.bias + n0 + c + k)));
+        const float z = tc_sigmoid(fmaf(acc[a + 32], inv_scale, __ldg(ep.bias + n0 + 64 + c + k)));
+        const float gin = fmaf(acc[a + 64], inv_scale, __ldg(ep.bias + n0 + 128 + c + k));
+        const float ghn = fmaf(acc[a + 96], inv_scale, __ldg(ep.bias + n0 + 192 + c + k));
+        const float n = tanhf(gin + r * ghn);
+        o[k] = (1.0f - z) * n + z * hv[k];
+      }
+      if (ep.dbg_nostore) continue;
+      *reinterpret_cast<float2*>(ep.c32 + orow * 256 + u) = make_float2(o[0], o[1]);
+      if (ep.out_hi) {
+        uint32_t lo;
+        const uint32_t hi = tc::split_pair_hi(o[0], o[1], &lo);
+        const size_t q = (size_t)row * ep.ldh + u;
+        *reinterpret_cast<uint32_t*>(ep.out_hi + q) = hi;
+        *reinterpret_cast<uint32_t*>(ep.out_lo + q) = lo;
+      }
+    }
+  }
+}
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, blockIdx.x + grid, ...
 // (n fastest, so CTAs running at the same time share A rows in L2).  The row count may live on the
 // device (ep.m_ptr, compacted human rows): no CTA is ever launched for an empty tile.  Rows are stored
@@ -474,7 +531,8 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
   constexpr int TC_A_TILE_BYTES = TcCfg<BN>::kATile;
   constexpr int TC_B_TILE_BYTES = TcCfg<BN>::kBTile;
   constexpr int TC_STAGE_BYTES = TcCfg<BN>::kStageBytes;
-  constexpr bool kTmaStore = !PROMOTE && BN == 256;
+  constexpr bool kTmaStore = !PROMOTE && BN == 256 && OUT != TC_OUT_GRU;
+  static_assert(OUT != TC_OUT_GRU || (BN == 256 && !PROMOTE), "the GRU epilogue reads four 64-column gate blocks");
   static_assert(!PROMOTE || BK == 64, "PROMOTE sums 64-wide k-blocks");
   static_assert(!kTmaStore || TcCfg<BN>::kStoreBoxes > 0, "BN = 256 stages its output");
   extern __shared__ uint8_t tc_smem_raw[];
@@ -628,7 +686,9 @@ cn_gemm_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
     TC_TRACE(const uint64_t t_loop = tc::globaltimer();)
     if constexpr (!PROMOTE) {
       TC_TRACE(const uint32_t waits0 = sg.waits; const uint64_t clk0 = sg.wait_clk;)
-      if constexpr (kTmaStore) {
+      if constexpr (OUT == TC_OUT_GRU) {
+        tc_epilogue_gru(acc, ep, inv_scale, n0, m0 + 64 * half + wr, cq, m_ext);
+      } else if constexpr (kTmaStore) {
         tc_epilogue_tma<ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half, wr, lane, sg, &map_c, &map_oh, &map_ol);
       } else {
         tc_epilogue_store<BN, ACT, OUT>(acc, ep, inv_scale, n0, m0 + 64 * half + wr, cq, m_ext);

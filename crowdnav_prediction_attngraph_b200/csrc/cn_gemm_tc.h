@@ -66,6 +66,15 @@ void gemm_tc(CnLaunchCtx* c, cudaStream_t st, const TcMat& A, const TcMat& B, in
              int act, const TcOut& o, const int* m_ptr = nullptr, int act_lo = 0, int act_hi = 1 << 30,
              const int* m0_ptr = nullptr);
 
+// One GRU cell step (hidden size 256, input size 64) over M rows as ONE GEMM with the gate math in the epilogue
+// (TC_OUT_GRU): A = [x (64) | m h (256)] split fp16 [M, 320]; B = the interleaved gate weights [1024, 320] (cn_dsrnn.cu),
+// bias [1024] in the same order.  h' of GEMM row r goes to the fp32 state row (r / group) * pitch + off + r % group of
+// h_out [*, 256]; h_in (same rows; null = zero state) times mask[r / group] is the previous state.  oh / ol (or null):
+// split fp16 copy of h' in GEMM row order, row pitch ldh.
+void gemm_tc_gru(CnLaunchCtx* c, cudaStream_t st, const TcMat& A, const TcMat& B, int M, const float* bias,
+                 const float* h_in, const float* mask, float* h_out, int group, int pitch, int off, __half* oh, __half* ol,
+                 int ldh);
+
 // The PPO update's GEMM (PROMOTE instance, BN = 64, plain launch on `st` with a grid of at most num_sms CTAs):
 // C[Mr, Nc] (+)= act((A_hi + A_lo)[Mr, Kd] (B_hi + B_lo)[Nc, Kd]^T * *inv_a * *inv_b + bias); Kd multiple of 64 in
 // storage (pitches), logical extents may be smaller (TMA zero-fills).  ksplit > 1: atomic adds into a zeroed C.

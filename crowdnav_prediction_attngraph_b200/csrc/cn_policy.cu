@@ -66,6 +66,15 @@ struct cn_policy {
   TcStoreMap qkv_st, sout_st;   // store maps of the fp32 outputs of the BN = 256 GEMMs (gemm_mode 1)
 };
 
+// The robot-human attention in its dense layout, for the DS-RNN forward (cn_dsrnn.cu): the kernel template is
+// defined, instantiated and launched in this translation unit only.
+void cn_hr_attention_dense(CnLaunchCtx* c, cudaStream_t st, const float* s_out, const float* u, const float* te, int ldte,
+                           int te_off, const float* b_s, int env_pitch, int env_off, int N, int H, float* wv,
+                           __half* wv_hi, __half* wv_lo, int ldwh) {
+  launch_k(c, cn_hr_attention_kernel<true>, dim3((N + 3) / 4), dim3(128), 0, st, s_out, u, te, ldte, te_off, b_s,
+           (const int*)nullptr, env_pitch, env_off, N, H, wv, wv_hi, wv_lo, ldwh);
+}
+
 namespace {
 
 int upload(cn_policy* p, float** dst, const std::vector<float>& src) {
@@ -484,8 +493,8 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   mark(p, st, 6);
   cudaStreamWaitEvent(st, p->ev_join, 0);
   mark(p, st, 7);
-  launch_k(&p->lc, cn_hr_attention_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->sout, p->u, p->t1, 128, 64, p->bs, p->row_start, N, H, p->wv,
-                                                      tcm ? p->tWv.hi : nullptr, tcm ? p->tWv.lo : nullptr);
+  launch_k(&p->lc, cn_hr_attention_kernel<false>, dim3((N + 3) / 4), dim3(128), 0, st, p->sout, p->u, p->t1, 128, 64, p->bs, p->row_start, 0, 0,
+                                                      N, H, p->wv, tcm ? p->tWv.hi : nullptr, tcm ? p->tWv.lo : nullptr, 256);
   // 3. GRU: emb overwrites the te half of t1 -> t1 = [enc | emb] = GRU input (gh came from the side stream)
   mark(p, st, 8);
   if (tcm) {

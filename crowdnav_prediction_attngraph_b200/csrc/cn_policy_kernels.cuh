@@ -486,19 +486,28 @@ __global__ void __launch_bounds__(W * 32) cn_hh_attention_kernel(const float* __
 //   score_j = <W_t robot + b_t, W_s s_j + b_s> * (H / sqrt(64))  ==  (u . s_j + cst) * H/8
 // with u = W_s^T te (precomputed by a GEMM), cst = <b_s, te>;  masked_fill(-1e9) for j >= n_e;
 // softmax over all H; weighted sum of the 256-d human features.
-__global__ void __launch_bounds__(128) cn_hr_attention_kernel(const float* __restrict__ s_out /* [N*H,256] */,
+// Row layouts of s_out (kDense): compacted (false: rows row_start[e] .. row_start[e + 1] - 1 of environment e, the
+// rest masked; env_pitch, env_off and ldwh unused, wv_hi / wv_lo have row pitch 256), or dense without a mask (true:
+// the H rows e * env_pitch + env_off + j, j < H, DS-RNN's spatial edge states inside its [N, H + 1, 256] edge state,
+// srnn_model.py:256-323; row_start unused, wv_hi / wv_lo have row pitch ldwh).  A template, so that the compacted
+// instance compiles to the same code as before the dense layout existed (a run-time switch cost 16 us per rollout
+// step at N = 4096, H = 20 on an H100).  cn_policy.cu launches the dense instance for cn_dsrnn.cu.
+template <bool kDense>
+__global__ void __launch_bounds__(128) cn_hr_attention_kernel(const float* __restrict__ s_out /* [*,256] */,
                                                               const float* __restrict__ u /* [N,256] */,
                                                               const float* __restrict__ te /* [N, ldte] cols te_off.. */,
                                                               int ldte, int te_off, const float* __restrict__ b_s,
-                                                              const int* __restrict__ row_start, int N, int H,
+                                                              const int* __restrict__ row_start, int env_pitch,
+                                                              int env_off, int N, int H,
                                                               float* __restrict__ wv /* [N,256] */,
-                                                              __half* __restrict__ wv_hi, __half* __restrict__ wv_lo) {
+                                                              __half* __restrict__ wv_hi, __half* __restrict__ wv_lo,
+                                                              int ldwh) {
   cn_pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int e = blockIdx.x * 4 + warp;
   if (e >= N) return;
-  const size_t row0 = (size_t)row_start[e];
-  const int n = row_start[e + 1] - row_start[e];
+  const size_t row0 = kDense ? (size_t)e * env_pitch + env_off : (size_t)row_start[e];
+  const int n = kDense ? H : row_start[e + 1] - row_start[e];
   float ur[8];
 #pragma unroll
   for (int t = 0; t < 8; ++t) ur[t] = u[(size_t)e * 256 + lane + 32 * t];
@@ -546,8 +555,9 @@ __global__ void __launch_bounds__(128) cn_hr_attention_kernel(const float* __res
     if (wv_hi) {
       const float c = fminf(fmaxf(acc[t], -65504.0f), 65504.0f);
       const __half hh = __float2half_rn(c);
-      wv_hi[o] = hh;
-      wv_lo[o] = __float2half_rn(c - __half2float(hh));
+      const size_t oh = (size_t)e * (kDense ? ldwh : 256) + lane + 32 * t;
+      wv_hi[oh] = hh;
+      wv_lo[oh] = __float2half_rn(c - __half2float(hh));
     }
   }
 }

@@ -51,6 +51,18 @@ def _summary(test_size, time_limit, end_codes, end_times, path_len, too_close_ra
     return out
 
 
+def _initial_hxs(actor_critic, n, dev):
+    """Zero recurrent state of n environments (rl/evaluation.py:16-21); the DS-RNN policy (base='srnn') also carries
+    its edge state [n, H+1, 256] from step to step, starting from an expanded zero (never materialised: the engine
+    takes it as the zero state)."""
+    hxs = {'human_node_rnn': torch.zeros(n, 1, 128, device=dev)}
+    if getattr(actor_critic, 'dsrnn', False):
+        b = actor_critic.base
+        hxs['human_human_edge_rnn'] = torch.zeros(1, 1, 1, device=dev).expand(n, b.human_num + 1,
+                                                                              b.human_human_edge_rnn_size)
+    return hxs
+
+
 def _act(actor_critic, obs, hxs, masks, n, dev):
     """(action, hxs): the policy's deterministic action and new recurrent state, or zeros for actor_critic=None (the
     ORCA / social-force robot baselines drive the robot inside env.step; the loop passes zeros, rl/evaluation.py:64-73)."""
@@ -68,7 +80,7 @@ def evaluate(actor_critic, eval_envs, num_processes, device, test_size, logging,
     dev = torch.device(device)
     time_limit = float(eval_envs.cfgd["time_limit"])
     dt = float(eval_envs.cfgd["time_step"])
-    hxs = {'human_node_rnn': torch.zeros(1, 1, 128, device=dev)}
+    hxs = _initial_hxs(actor_critic, 1, dev)
     masks = torch.zeros(1, 1, device=dev)
     end_codes, end_times, all_path_len, too_close_ratios, min_dist, ep_rewards, steps = [], [], [], [], [], [], []
     for k in range(test_size):
@@ -160,7 +172,7 @@ def evaluate_batched(actor_critic, config, env_name, seed, test_size, device, lo
     if int(d.get("robot_policy", 0)) == 1:
         _freeze_robot_sim(base, d, dev)
     time_limit, dt = float(d["time_limit"]), float(d["time_step"])
-    hxs = {'human_node_rnn': torch.zeros(N, 1, 128, device=dev)}
+    hxs = _initial_hxs(actor_critic, N, dev)
     masks = torch.zeros(N, 1, device=dev)
     obs = env.reset()
     last_pos = obs['robot_node'][:, 0, :2].cpu().numpy()

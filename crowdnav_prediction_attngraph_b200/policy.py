@@ -90,20 +90,24 @@ class CudaPolicy(object):
     """Thin handle on cn_policy: upload a reference state_dict, run the rollout forward."""
 
     def __init__(self, num_envs, human_num, input_size=12, device="cuda:0", gemm_mode=1):
-        self.lib = _capi.load_library()
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("CudaPolicy needs a CUDA device (no CPU fallback)")
-        self.N, self.H, self.Win = num_envs, human_num, input_size
+        self._setup(num_envs, human_num, input_size, device)
         cfg = _capi.CnPolicyConfig(num_envs, human_num, input_size,
                                    self.device.index if self.device.index is not None else 0, gemm_mode)
         self._h = C.c_void_p()
         _capi.check(self.lib, self.lib.cn_policy_create(C.byref(cfg), C.byref(self._h)), "cn_policy_create")
-        dev = self.device
+
+    def _setup(self, num_envs, human_num, input_size, device, **extra_outputs):
+        """What every engine handle holds: the library, the device (CUDA only), the sizes, the two output buffers that
+        act() alternates between (value, action, log_prob, h_out, mean and `extra_outputs` {name: shape}) and the noise
+        generator state."""
+        self.lib = _capi.load_library()
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise RuntimeError("%s needs a CUDA device (no CPU fallback)" % type(self).__name__)
+        self.N, self.H, self.Win = num_envs, human_num, input_size
         N = num_envs
-        self._bufs = [dict(value=torch.zeros(N, 1, device=dev), action=torch.zeros(N, 2, device=dev),
-                           log_prob=torch.zeros(N, 1, device=dev), h_out=torch.zeros(N, 1, HIDDEN, device=dev),
-                           mean=torch.zeros(N, 2, device=dev)) for _ in range(2)]
+        shapes = dict(value=(N, 1), action=(N, 2), log_prob=(N, 1), h_out=(N, 1, HIDDEN), mean=(N, 2), **extra_outputs)
+        self._bufs = [{k: torch.zeros(*shp, device=self.device) for k, shp in shapes.items()} for _ in range(2)]
         self._flip = 0
         self._gen = None
 
@@ -120,20 +124,28 @@ class CudaPolicy(object):
         with torch.cuda.device(self.device):
             _capi.check(self.lib, self.lib.cn_policy_finalize(self._h, self._stream()), "cn_policy_finalize")
 
-    def act(self, obs, h, masks, deterministic=False, return_mean=False, noise=None, out=None):
-        """obs: dict of device tensors; h: [N,1,128]; masks: [N,1].  Returns value, action, log_prob, h_new
-        (views of internal double buffers: valid until the call after next).  `out` (optional dict with
-        contiguous float32 device tensors value/action/log_prob/h_out) makes the kernels write straight
-        into caller memory, e.g. the rollout-storage slot (zero-copy rollout)."""
-        N = self.N
+    def _outputs(self, out, keys=("value", "action", "log_prob", "h_out")):
+        """The next of the two internal output buffers, with the entries of `out` (caller memory) in their place."""
         self._flip ^= 1
         b = self._bufs[self._flip]
         if out is not None:
             b = dict(b)
-            for k in ("value", "action", "log_prob", "h_out"):
+            for k in keys:
                 if k in out:
                     assert out[k].is_cuda and out[k].is_contiguous() and out[k].dtype == torch.float32, k
                     b[k] = out[k]
+        return b
+
+    def _inputs(self, **args):
+        f32, dev = torch.float32, self.device
+        for k, t in args.items():
+            if t.dtype is not f32 or not t.is_contiguous() or t.device != dev:
+                args[k] = t.to(dev, f32).contiguous()
+        return args
+
+    def _noise(self, deterministic, noise):
+        """Standard normal action noise [N, 2] for this step (None when deterministic)."""
+        N = self.N
         if not deterministic and noise is None:
             # torch.normal(mean, std) == randn * std + mean.  Data-parallel replicas are seeded alike by train.py
             # (identical initial weights): give every rank its own noise stream so their actions decorrelate.
@@ -152,13 +164,18 @@ class CudaPolicy(object):
                 self._noise_state = (g.initial_seed(), g.get_offset())
             noise = nb[self._noise_i]
             self._noise_i += 1
-        sp = obs["spatial_edges"]
-        args = dict(robot_node=obs["robot_node"], temporal_edges=obs["temporal_edges"], spatial_edges=sp,
-                    detected_human_num=obs["detected_human_num"], h_in=h, masks=masks)
-        f32, dev = torch.float32, self.device
-        for k, t in args.items():
-            if t.dtype is not f32 or not t.is_contiguous() or t.device != dev:
-                args[k] = t.to(dev, f32).contiguous()
+        return noise
+
+    def act(self, obs, h, masks, deterministic=False, return_mean=False, noise=None, out=None):
+        """obs: dict of device tensors; h: [N,1,128]; masks: [N,1].  Returns value, action, log_prob, h_new
+        (views of internal double buffers: valid until the call after next).  `out` (optional dict with
+        contiguous float32 device tensors value/action/log_prob/h_out) makes the kernels write straight
+        into caller memory, e.g. the rollout-storage slot (zero-copy rollout)."""
+        b = self._outputs(out)
+        noise = self._noise(deterministic, noise)
+        args = self._inputs(robot_node=obs["robot_node"], temporal_edges=obs["temporal_edges"],
+                            spatial_edges=obs["spatial_edges"], detected_human_num=obs["detected_human_num"],
+                            h_in=h, masks=masks)
         ptrs = _capi.CnActPtrs(
             args["robot_node"].data_ptr(), args["temporal_edges"].data_ptr(), args["spatial_edges"].data_ptr(),
             args["detected_human_num"].data_ptr(), args["h_in"].data_ptr(), args["masks"].data_ptr(),
@@ -187,6 +204,138 @@ class CudaPolicy(object):
             pass
 
 
+EDGE = 256                # human_human_edge_rnn_size
+DSRNN_UNUSED = ("base.humanNodeRNN.edge_embed.", "base.human_node_final_linear.", "base.spatial_linear.")
+
+
+def _is_zero_view(t):
+    """An expanded scalar (every stride 0): the all-zero edge state the rollout storage keeps for a policy without
+    a recurrent edge state.  The kernels take it as a NULL pointer, so it is never materialised."""
+    return t is None or (t.dim() > 0 and all(s == 0 for s in t.stride()))
+
+
+class CudaDsrnn(CudaPolicy):
+    """Thin handle on cn_dsrnn (the DS-RNN forward); noise and output buffers as CudaPolicy."""
+
+    def __init__(self, num_envs, human_num, input_size=2, device="cuda:0"):
+        self._setup(num_envs, human_num, input_size, device, edge_h_out=(num_envs, human_num + 1, EDGE))
+        cfg = _capi.CnDsrnnConfig(num_envs, human_num, input_size, self.device.index if self.device.index is not None else 0)
+        self._h = C.c_void_p()
+        _capi.check(self.lib, self.lib.cn_dsrnn_create(C.byref(cfg), C.byref(self._h)), "cn_dsrnn_create")
+
+    def load_state_dict(self, sd):
+        for k, v in sd.items():
+            if k.startswith(DSRNN_UNUSED):
+                continue
+            arr = v.detach().to("cpu", torch.float32).contiguous().numpy()
+            _capi.check(self.lib, self.lib.cn_dsrnn_set_param(self._h, k.encode(), arr.ctypes.data, arr.size),
+                        "cn_dsrnn_set_param(%s)" % k)
+        with torch.cuda.device(self.device):
+            _capi.check(self.lib, self.lib.cn_dsrnn_finalize(self._h, self._stream()), "cn_dsrnn_finalize")
+
+    def act(self, obs, h, edge_h, masks, deterministic=False, return_mean=False, noise=None, out=None):
+        """As CudaPolicy.act, plus the edge state: edge_h [N,H+1,256] (None or an expanded zero: zero state) in,
+        edge_h_out out (also an `out` key).  Returns value, action, log_prob, h_new, edge_h_new (, mean)."""
+        b = self._outputs(out, ("value", "action", "log_prob", "h_out", "edge_h_out"))
+        noise = self._noise(deterministic, noise)
+        args = self._inputs(robot_node=obs["robot_node"], temporal_edges=obs["temporal_edges"],
+                            spatial_edges=obs["spatial_edges"], h_in=h, masks=masks)
+        if not _is_zero_view(edge_h):
+            args.update(self._inputs(edge_h_in=edge_h))
+        eh = args.get("edge_h_in")
+        ptrs = _capi.CnDsrnnActPtrs(
+            args["robot_node"].data_ptr(), args["temporal_edges"].data_ptr(), args["spatial_edges"].data_ptr(),
+            args["h_in"].data_ptr(), None if eh is None else eh.data_ptr(), args["masks"].data_ptr(),
+            None if deterministic else noise.data_ptr(), b["value"].data_ptr(), b["action"].data_ptr(),
+            b["log_prob"].data_ptr(), b["h_out"].data_ptr(), b["edge_h_out"].data_ptr(), b["mean"].data_ptr())
+        rc = self.lib.cn_dsrnn_act(self._h, C.byref(ptrs), self._stream())
+        if rc:
+            _capi.check(self.lib, rc, "cn_dsrnn_act")
+        self._keep = (args, noise)
+        res = (b["value"], b["action"], b["log_prob"], b["h_out"], b["edge_h_out"])
+        return res + (b["mean"],) if return_mean else res
+
+    def launch_count(self):
+        return int(self.lib.cn_dsrnn_launch_count(self._h))
+
+    def stage_ms(self):
+        """{stage: ms} of the last act (profiling must have been enabled with profile(True) before it)."""
+        n = self.lib.cn_dsrnn_stage_count()
+        out = (C.c_float * n)()
+        _capi.check(self.lib, self.lib.cn_dsrnn_stage_ms(self._h, out, n), "cn_dsrnn_stage_ms")
+        return {self.lib.cn_dsrnn_stage_name(i).decode(): float(out[i]) for i in range(n)}
+
+    def profile(self, enable=True):
+        _capi.check(self.lib, self.lib.cn_dsrnn_profile(self._h, int(enable)), "cn_dsrnn_profile")
+
+    def close(self):
+        if self._h:
+            self.lib.cn_dsrnn_destroy(self._h)
+            self._h = None
+
+
+class _SrnnParams(nn.Module):
+    """Parameter container with the reference SRNN's module tree (srnn_model.py:326-387) and initialisers."""
+
+    def __init__(self, input_size):
+        super().__init__()
+        g = math.sqrt(2)
+
+        def gru(i, h):
+            m = nn.GRU(i, h)
+            for name, prm in m.named_parameters():                 # srnn_model.py:26-30
+                if 'bias' in name:
+                    nn.init.constant_(prm, 0)
+                else:
+                    nn.init.orthogonal_(prm)
+            return m
+
+        def edge_rnn(w):
+            e = nn.Module()
+            e.gru = gru(64, EDGE)
+            e.encoder_linear = nn.Linear(w, 64)
+            return e
+        base = nn.Module()
+        node = nn.Module()
+        node.gru = gru(128, HIDDEN)
+        node.encoder_linear = nn.Linear(3, 64)
+        node.edge_embed = nn.Linear(EDGE, 64)                      # unused by the forward
+        node.edge_attention_embed = nn.Linear(2 * EDGE, 64)
+        node.output_linear = nn.Linear(HIDDEN, 256)
+        base.humanNodeRNN = node
+        base.humanhumanEdgeRNN_spatial = edge_rnn(input_size)
+        base.humanhumanEdgeRNN_temporal = edge_rnn(2)
+        att = nn.Module()
+        att.temporal_edge_layer = nn.ModuleList([nn.Linear(EDGE, 64)])
+        att.spatial_edge_layer = nn.ModuleList([nn.Linear(EDGE, 64)])
+        base.attn = att
+        base.actor = nn.Sequential(_ortho(nn.Linear(256, 256), g), nn.Tanh(), _ortho(nn.Linear(256, 256), g), nn.Tanh())
+        base.critic = nn.Sequential(_ortho(nn.Linear(256, 256), g), nn.Tanh(), _ortho(nn.Linear(256, 256), g), nn.Tanh())
+        base.critic_linear = _ortho(nn.Linear(256, 1), g)
+        base.robot_linear = _ortho(nn.Linear(7, 3), g)
+        base.human_node_final_linear = _ortho(nn.Linear(256, 2), g)   # unused by the forward
+        base.spatial_linear = _ortho(nn.Linear(input_size, 2), g)     # unused by the forward
+        self.base = base
+        dist = nn.Module()
+        dist.fc_mean = _ortho(nn.Linear(256, 2))
+        dist.logstd = _AddBias(2)
+        self.dist = dist
+
+
+def _gru_masked(gru, x, h, masks, rep):
+    """RNNBase._forward_gru (srnn_model.py:50-103) over [T, B, in] with done masks [T, n] (B = n * rep rows): the
+    sequence is cut where any mask is 0, and each segment starts from h * mask.  Returns outputs [T, B, hid], h."""
+    T = x.shape[0]
+    cuts = [0] + [t + 1 for t in (masks[1:] == 0).any(-1).nonzero().flatten().tolist()] + [T]
+    outs = []
+    for a, b in zip(cuts[:-1], cuts[1:]):
+        h = h * masks[a].repeat_interleave(rep)[:, None]
+        y, h1 = gru(x[a:b], h[None])
+        h = h1[0]
+        outs.append(y)
+    return torch.cat(outs, 0), h
+
+
 def _hh_attention(q, k, v, valid):
     """softmax(q k^T / 8 + key mask) v for [B, 8, H, 64] tensors with H <= ~20 keys.  Written as two batched
     matmuls: at this shape the fused 'memory efficient' SDPA kernels (64 x 64 tiles for a 20-key sequence) cost
@@ -203,15 +352,22 @@ class Policy(nn.Module):
 
     def __init__(self, obs_shape, action_space, base=None, base_kwargs=None):
         super().__init__()
-        if base not in (None, 'selfAttn_merge_srnn'):
-            raise NotImplementedError("only base='selfAttn_merge_srnn' is on the hot path (SURVEY.md §2.1 row 9)")
+        if base not in (None, 'selfAttn_merge_srnn', 'srnn'):
+            raise NotImplementedError("base=%r: the engine runs 'selfAttn_merge_srnn' and 'srnn'" % (base,))
+        args = base_kwargs
+        self.dsrnn = base == 'srnn'
+        if self.dsrnn:
+            # The reference reads args.env_type (srnn_model.py:378), which arguments.py never defines; 'crowd_sim' is
+            # the only value whose robot_linear input width (7) matches robot_node, so a missing env_type means it.
+            env_type = getattr(args, 'env_type', 'crowd_sim') if args is not None else 'crowd_sim'
+            if env_type != 'crowd_sim':
+                raise NotImplementedError("base='srnn' runs env_type 'crowd_sim' only (got %r)" % (env_type,))
         sp = obs_shape['spatial_edges'].shape
         self.human_num, self.input_size = int(sp[0]), int(sp[1])
-        args = base_kwargs
         self.nenv = int(getattr(args, 'num_processes', 1)) if args is not None else 1
         self.seq_length = int(getattr(args, 'seq_length', 30)) if args is not None else 30
         self.nminibatch = int(getattr(args, 'num_mini_batch', 2)) if args is not None else 2
-        p = _Params(self.input_size)
+        p = (_SrnnParams if self.dsrnn else _Params)(self.input_size)
         self.base = p.base
         # attributes the reference's callers read / write on `actor_critic.base` (test.py:148, rl/evaluation.py:15-21)
         self.base.nenv = self.nenv
@@ -234,8 +390,11 @@ class Policy(nn.Module):
     # ------------------------------------------------------------------ CUDA rollout path
     def _engine(self, N, device):
         if self._cuda is None or self._cuda.N != N or self._cuda.device != device:
-            self._cuda = CudaPolicy(N, self.human_num, self.input_size, device=device,
-                                    gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")))
+            if self.dsrnn:
+                self._cuda = CudaDsrnn(N, self.human_num, self.input_size, device=device)
+            else:
+                self._cuda = CudaPolicy(N, self.human_num, self.input_size, device=device,
+                                        gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")))
             self._cuda_version = -1
         # parameter objects are fixed after construction: walk the module tree once, then only read the
         # version counters (the tree walk alone cost ~0.1 ms of host time per act)
@@ -255,6 +414,11 @@ class Policy(nn.Module):
     def act(self, inputs, rnn_hxs, masks, deterministic=False):
         sp = inputs['spatial_edges']
         eng = self._engine(sp.shape[0], sp.device)
+        if self.dsrnn:
+            value, action, logp, h_new, e_new = eng.act(inputs, rnn_hxs['human_node_rnn'],
+                                                        rnn_hxs.get('human_human_edge_rnn'), masks,
+                                                        deterministic=deterministic)
+            return value, action, logp, {'human_node_rnn': h_new, 'human_human_edge_rnn': e_new}
         value, action, logp, h_new = eng.act(inputs, rnn_hxs['human_node_rnn'], masks, deterministic=deterministic)
         z = self.__dict__.get("_zero_edge")
         if z is None or z.device != sp.device or z.shape[0] != sp.shape[0]:
@@ -266,6 +430,9 @@ class Policy(nn.Module):
     def get_value(self, inputs, rnn_hxs, masks):
         sp = inputs['spatial_edges']
         eng = self._engine(sp.shape[0], sp.device)
+        if self.dsrnn:
+            return eng.act(inputs, rnn_hxs['human_node_rnn'], rnn_hxs.get('human_human_edge_rnn'), masks,
+                           deterministic=True)[0]
         value, _, _, _ = eng.act(inputs, rnn_hxs['human_node_rnn'], masks, deterministic=True)
         return value
 
@@ -396,12 +563,43 @@ class Policy(nn.Module):
         ha = torch.tanh(lin(torch.tanh(lin(y, b.actor[0])), b.actor[2]))
         return b.critic_linear(hc), ha, h.reshape(N, 1, HIDDEN)
 
+    def _features_dsrnn(self, inputs, hxs, masks, T, N):
+        """SRNN.forward with infer=False (srnn_model.py:389-468) over a [T, N] minibatch: PyTorch ops (cuDNN GRUs on
+        a CUDA device).  hxs: node state [N,1,128] and edge state [N,H+1,256] (an expanded zero is fine)."""
+        b = self.base
+        H = self.human_num
+        m = masks.reshape(T, N)
+        he = hxs['human_human_edge_rnn'].reshape(N, H + 1, EDGE)
+        et, es = b.humanhumanEdgeRNN_temporal, b.humanhumanEdgeRNN_spatial
+        xt = torch.relu(et.encoder_linear(inputs['temporal_edges'].reshape(T, N, 2)))
+        ht, ht_last = _gru_masked(et.gru, xt, he[:, 0], m, 1)                          # [T, N, 256]
+        xs = torch.relu(es.encoder_linear(inputs['spatial_edges'].reshape(T, N * H, -1)))
+        hs, hs_last = _gru_masked(es.gru, xs, he[:, 1:].reshape(N * H, EDGE), m, H)   # [T, N H, 256]
+        hs = hs.reshape(T, N, H, EDGE)
+        te = b.attn.temporal_edge_layer[0](ht)
+        se = b.attn.spatial_edge_layer[0](hs)
+        p = torch.softmax((te[:, :, None, :] * se).sum(-1) * (H / 8.0), dim=-1)
+        wv = torch.matmul(p[:, :, None, :], hs).squeeze(2)                             # [T, N, 256]
+        nr = b.humanNodeRNN
+        enc = torch.relu(nr.encoder_linear(b.robot_linear(inputs['robot_node'].reshape(T, N, 7))))
+        emb = torch.relu(nr.edge_attention_embed(torch.cat([ht, wv], -1)))
+        hn, hn_last = _gru_masked(nr.gru, torch.cat([enc, emb], -1), hxs['human_node_rnn'].reshape(N, HIDDEN), m, 1)
+        x = nr.output_linear(hn).reshape(T * N, 256)
+        edge = torch.cat([ht_last[:, None], hs_last.reshape(N, H, EDGE)], 1)
+        return b.critic_linear(b.critic(x)), b.actor(x), {'human_node_rnn': hn_last.reshape(N, 1, HIDDEN),
+                                                         'human_human_edge_rnn': edge}
+
     def evaluate_actions(self, inputs, rnn_hxs, masks, action):
-        """inputs flattened [T*N, ...] (storage.py recurrent_generator), rnn_hxs['human_node_rnn'] [N,1,128]."""
+        """inputs flattened [T*N, ...] (storage.py recurrent_generator), rnn_hxs['human_node_rnn'] [N,1,128]
+        (DS-RNN: and rnn_hxs['human_human_edge_rnn'] [N,H+1,256])."""
         h0 = rnn_hxs['human_node_rnn']
         N = h0.shape[0]
         T = inputs['spatial_edges'].shape[0] // N
-        value, feat, h = self._features(inputs, h0, masks, T, N)
+        if self.dsrnn:
+            value, feat, hxs = self._features_dsrnn(inputs, rnn_hxs, masks, T, N)
+        else:
+            value, feat, h = self._features(inputs, h0, masks, T, N)
+            hxs = {'human_node_rnn': h}
         mean = self.dist.fc_mean(feat)
         logstd = self.dist.logstd._bias.t().view(1, -1).expand_as(mean)
         dist = torch.distributions.Normal(mean, logstd.exp())
@@ -409,4 +607,4 @@ class Policy(nn.Module):
         # the reference's FixedNormal defines `entrop` (typo, distributions.py:42), so model.py:88 reaches
         # torch's Normal.entropy() -> [B, 2] and .mean() averages over BOTH action dimensions
         entropy = dist.entropy().mean()
-        return value, logp, entropy, {'human_node_rnn': h}
+        return value, logp, entropy, hxs

@@ -2,12 +2,16 @@
 (rl/networks/storage.py:13-253): obs{} / recurrent_hidden_states{} / masks / insert /
 compute_returns (GAE) / after_update / recurrent_generator — everything stays on the GPU.
 
-Differences that do not change results: tensors are created directly on `device`; the all-zero
-`human_human_edge_rnn` hidden state (2.7 GB at N=4096, H=20 in the reference, storage.py:34) is a
-stride-0 expanded zero; `recurrent_generator` gathers minibatches with one index_select per
-tensor instead of a Python loop over environments (storage.py:208-223)."""
+Differences that do not change results: tensors are created directly on `device`; the
+`human_human_edge_rnn` hidden state (2.7 GB at N=4096, H=20 in the reference, storage.py:34) starts as a
+stride-0 expanded zero, which is all the attention-graph policy ever stores there; the first `insert` of a
+real edge state (the DS-RNN policy, base='srnn') replaces it with a [T+1, N, H+1, 256] buffer;
+`recurrent_generator` gathers minibatches with one index_select per tensor instead of a Python loop over
+environments (storage.py:208-223)."""
 
 import torch
+
+from .policy import CudaDsrnn, _is_zero_view
 
 
 class RolloutStorage(object):
@@ -46,21 +50,35 @@ class RolloutStorage(object):
         hn = self.recurrent_hidden_states
         hn['human_node_rnn'] = hn['human_node_rnn'].to(dev)
         e = hn['human_human_edge_rnn']
-        hn['human_human_edge_rnn'] = torch.zeros(1, 1, 1, 1, device=dev).expand(*e.shape)
+        hn['human_human_edge_rnn'] = e.to(dev) if self._edge_real() else torch.zeros(1, 1, 1, 1, device=dev).expand(*e.shape)
         for name in ("rewards", "value_preds", "returns", "action_log_probs", "actions", "masks", "bad_masks"):
             setattr(self, name, getattr(self, name).to(dev))
         self.device = dev
 
+    def _edge_real(self):
+        return self.recurrent_hidden_states['human_human_edge_rnn'].stride()[0] != 0
+
+    def _edge_materialise(self):
+        """Switch to a real (zero-filled) edge-state buffer; called the first time a recurrent edge state arrives."""
+        if self._edge_real():
+            return
+        e = self.recurrent_hidden_states['human_human_edge_rnn']
+        self.recurrent_hidden_states['human_human_edge_rnn'] = torch.zeros(*e.shape, device=self.device)
+        self.__dict__.pop("_slots", None)
+
+    def _dsts(self, s):
+        dst = [self.obs[key][s + 1] for key in self.obs]
+        dst += [self.recurrent_hidden_states['human_node_rnn'][s + 1], self.actions[s], self.action_log_probs[s],
+                self.value_preds[s], self.rewards[s], self.masks[s + 1], self.bad_masks[s + 1]]
+        if self._edge_real():
+            dst.append(self.recurrent_hidden_states['human_human_edge_rnn'][s + 1])
+        return dst
+
     def _slot_table(self):
         """Per step index: the destination tensors of insert() with their device pointers and byte sizes, built once per
-        device (the storage tensors are never reallocated except by .to(), which drops the table)."""
-        tab = []
-        for s in range(self.num_steps):
-            dst = [self.obs[key][s + 1] for key in self.obs]
-            dst += [self.recurrent_hidden_states['human_node_rnn'][s + 1], self.actions[s], self.action_log_probs[s],
-                    self.value_preds[s], self.rewards[s], self.masks[s + 1], self.bad_masks[s + 1]]
-            tab.append([(d, d.data_ptr(), d.numel() * d.element_size()) for d in dst])
-        return tab
+        device (the storage tensors are never reallocated except by .to() and the switch to a real edge state, which
+        drop the table)."""
+        return [[(d, d.data_ptr(), d.numel() * d.element_size()) for d in self._dsts(s)] for s in range(self.num_steps)]
 
     def insert(self, obs, recurrent_hidden_states, actions, action_log_probs, value_preds, rewards, masks, bad_masks=None):
         """rl/networks/storage.py:70-86.  Every source that the GPU can read directly -- device tensors (observations,
@@ -68,13 +86,15 @@ class RolloutStorage(object):
         -- is copied by ONE cn_copy_segments launch instead of twelve torch copy_ calls; pageable host tensors (what the
         reference's train.py builds) take the usual H2D copy_."""
         s = self.step
+        edge = recurrent_hidden_states.get('human_human_edge_rnn')
+        if not _is_zero_view(edge):
+            self._edge_materialise()
         srcs = [obs[key] for key in self.obs]
         srcs += [recurrent_hidden_states['human_node_rnn'], actions, action_log_probs, value_preds, rewards, masks, bad_masks]
+        if self._edge_real():
+            srcs.append(edge)
         if self.device.type != "cuda":
-            dsts = [self.obs[key][s + 1] for key in self.obs]
-            dsts += [self.recurrent_hidden_states['human_node_rnn'][s + 1], self.actions[s], self.action_log_probs[s],
-                     self.value_preds[s], self.rewards[s], self.masks[s + 1], self.bad_masks[s + 1]]
-            for dst, src in zip(dsts, srcs):
+            for dst, src in zip(self._dsts(s), srcs):
                 if src is not None:
                     dst.copy_(src.reshape(dst.shape) if src.numel() == dst.numel() else src)
             self.step = (s + 1) % self.num_steps
@@ -115,9 +135,15 @@ class RolloutStorage(object):
         s = self.step
         o = {k: v[s] for k, v in self.obs.items()}
         hn = self.recurrent_hidden_states['human_node_rnn']
-        engine.act(o, hn[s], self.masks[s], deterministic=deterministic,
-                   out=dict(value=self.value_preds[s], action=self.actions[s], log_prob=self.action_log_probs[s],
-                            h_out=hn[s + 1]))
+        out = dict(value=self.value_preds[s], action=self.actions[s], log_prob=self.action_log_probs[s], h_out=hn[s + 1])
+        if isinstance(engine, CudaDsrnn):
+            # the DS-RNN engine carries the edge state: its kernels write slot s + 1 of a real buffer
+            self._edge_materialise()
+            he = self.recurrent_hidden_states['human_human_edge_rnn']
+            out["edge_h_out"] = he[s + 1]
+            engine.act(o, hn[s], he[s], self.masks[s], deterministic=deterministic, out=out)
+        else:
+            engine.act(o, hn[s], self.masks[s], deterministic=deterministic, out=out)
         env.step_device(self.actions[s], obs_out={k: v[s + 1] for k, v in self.obs.items()},
                         reward_out=self.rewards[s], not_done_out=self.masks[s + 1])
         self.step = (s + 1) % self.num_steps
@@ -126,6 +152,8 @@ class RolloutStorage(object):
         for key in self.obs:
             self.obs[key][0].copy_(self.obs[key][-1])
         self.recurrent_hidden_states['human_node_rnn'][0].copy_(self.recurrent_hidden_states['human_node_rnn'][-1])
+        if self._edge_real():
+            self.recurrent_hidden_states['human_human_edge_rnn'][0].copy_(self.recurrent_hidden_states['human_human_edge_rnn'][-1])
         self.masks[0].copy_(self.masks[-1])
         self.bad_masks[0].copy_(self.bad_masks[-1])
 
@@ -157,7 +185,8 @@ class RolloutStorage(object):
             ind = perm[start:start + per]
             flat = lambda x: x.index_select(1, ind).reshape(T * per, *x.shape[2:])
             obs_batch = {k: flat(v[:-1]) for k, v in self.obs.items()}
+            he = self.recurrent_hidden_states['human_human_edge_rnn']
             hxs = {'human_node_rnn': self.recurrent_hidden_states['human_node_rnn'][0].index_select(0, ind),
-                   'human_human_edge_rnn': self.recurrent_hidden_states['human_human_edge_rnn'][0, :per]}
+                   'human_human_edge_rnn': he[0].index_select(0, ind) if self._edge_real() else he[0, :per]}
             yield (obs_batch, hxs, flat(self.actions), flat(self.value_preds[:-1]), flat(self.returns[:-1]),
                    flat(self.masks[:-1]), flat(self.action_log_probs), flat(advantages))

@@ -222,6 +222,49 @@ const char *cn_policy_stage_name(int i);
 int cn_policy_stage_ms(cn_policy *pol, float *out, int n);
 
 /* ------------------------------------------------------------------------------------------ */
+/* DS-RNN policy (the reference's base = 'srnn': rl/networks/srnn_model.py:326-468), rollout forward only.
+ * Tensor-core path only (there is no gemm_mode).  Parameters by the reference's state_dict keys; the six tensors the
+ * forward never reads (humanNodeRNN.edge_embed.*, human_node_final_linear.*, spatial_linear.*) need not be set.    */
+
+typedef struct cn_dsrnn cn_dsrnn;
+
+typedef struct cn_dsrnn_config {
+  int32_t num_envs;     /* N                                                                   */
+  int32_t human_num;    /* H                                                                   */
+  int32_t input_size;   /* spatial_edges row width W (2 for VarNum, 12 for Pred envs)          */
+  int32_t device;
+} cn_dsrnn_config;
+
+int cn_dsrnn_create(const cn_dsrnn_config *cfg, cn_dsrnn **out);
+int cn_dsrnn_destroy(cn_dsrnn *pol);
+int cn_dsrnn_set_param(cn_dsrnn *pol, const char *key, const float *h_data, size_t count);
+int cn_dsrnn_finalize(cn_dsrnn *pol, void *stream);
+
+typedef struct cn_dsrnn_act_ptrs {
+  /* inputs */
+  const float *robot_node, *temporal_edges, *spatial_edges;   /* [N,1,7], [N,1,2], [N,H,W]                    */
+  const float *h_in;        /* rnn_hxs['human_node_rnn'] [N,1,128]                                            */
+  const float *edge_h_in;   /* rnn_hxs['human_human_edge_rnn'] [N,H+1,256], or NULL for an all-zero state      */
+  const float *masks;       /* [N,1]                                                                          */
+  const float *noise;       /* [N,2] standard normal draws, or NULL for deterministic (mode)                  */
+  /* outputs */
+  float *value, *action, *log_prob;   /* [N,1], [N,2], [N,1]                                                 */
+  float *h_out;             /* [N,1,128]                                                                      */
+  float *edge_h_out;        /* [N,H+1,256]: row 0 the temporal edge state, rows 1..H the spatial ones          */
+  float *action_mean;       /* [N,2] or NULL                                                                  */
+} cn_dsrnn_act_ptrs;
+
+/* replaces: Policy.act (rl/networks/model.py:56-74) with base = 'srnn', infer=True.  edge_h_out must not overlap
+ * h_in / edge_h_in other than being equal to edge_h_in (in-place update).                                        */
+int cn_dsrnn_act(cn_dsrnn *pol, const cn_dsrnn_act_ptrs *d, void *stream);
+int64_t cn_dsrnn_launch_count(cn_dsrnn *pol);
+/* per-stage device timing, as cn_policy_profile / cn_policy_stage_ms                                             */
+int cn_dsrnn_profile(cn_dsrnn *pol, int enable);
+int cn_dsrnn_stage_count(void);
+const char *cn_dsrnn_stage_name(int i);
+int cn_dsrnn_stage_ms(cn_dsrnn *pol, float *out, int n);
+
+/* ------------------------------------------------------------------------------------------ */
 /* PPO update path (rl/ppo/ppo.py:36-101 -> Policy.evaluate_actions, selfAttn_srnn_temp_node.py:63-91): the
  * per-human linear layers forward / backward on the wgmma 3xFP16 GEMM in fp32-equivalent accuracy.
  * Stateless: every buffer (outputs, `d_saved` = what the backward needs from the forward, workspace) is caller-owned
