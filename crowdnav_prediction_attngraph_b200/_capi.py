@@ -74,6 +74,8 @@ EXPORTS = [
     "cn_update_attn_fwd", "cn_update_attn_bwd", "cn_update_gru_fwd", "cn_update_gru_bwd",
     "cn_dsrnn_create", "cn_dsrnn_destroy", "cn_dsrnn_set_param", "cn_dsrnn_finalize", "cn_dsrnn_act",
     "cn_dsrnn_launch_count", "cn_dsrnn_profile", "cn_dsrnn_stage_count", "cn_dsrnn_stage_name", "cn_dsrnn_stage_ms",
+    "cn_env_create_collect", "cn_env_reset_collect", "cn_env_step_collect", "cn_recorder_create", "cn_recorder_destroy",
+    "cn_recorder_append", "cn_recorder_pending", "cn_recorder_flush", "cn_write_rows_txt", "cn_format_rows",
 ]
 
 _lib = None
@@ -187,6 +189,17 @@ def load_library(path=None):
     lib.cn_update_attn_bwd.argtypes = [C.c_void_p] * 6 + [C.c_int] + [C.c_void_p] * 2 + [C.c_int, C.c_void_p]
     lib.cn_update_gru_fwd.argtypes = [C.c_void_p] * 5 + [C.c_int] * 2 + [C.c_void_p] * 2 + [C.c_int, C.c_void_p]
     lib.cn_update_gru_bwd.argtypes = [C.c_void_p] * 7 + [C.c_int] * 2 + [C.c_void_p] * 3 + [C.c_int, C.c_void_p]
+    lib.cn_env_create_collect.argtypes = [C.POINTER(CnConfig), C.POINTER(C.c_void_p)]
+    lib.cn_env_reset_collect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.cn_env_step_collect.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(CnStepPtrs), C.c_void_p]
+    lib.cn_recorder_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
+    lib.cn_recorder_destroy.argtypes = [C.c_void_p]
+    lib.cn_recorder_append.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.cn_recorder_pending.argtypes = [C.c_void_p]
+    lib.cn_recorder_flush.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]
+    lib.cn_write_rows_txt.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    lib.cn_format_rows.restype = C.c_int64
+    lib.cn_format_rows.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
     if path is None:
         _lib = lib
     return lib

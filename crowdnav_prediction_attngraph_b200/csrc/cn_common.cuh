@@ -54,6 +54,8 @@ struct CnParams {
   int defer_tries;        // warp-scope rejection-sampling budget (cn_env_event_kernel -> cn_env_event_heavy_kernel)
   int robot_policy;       // robot.policy: 0 caller's action, 1 'orca', 2 'social_force' (cn_robot_act)
   int robot_visible;      // robot.visible: the humans' solves take the robot as one more agent (cn_orca_build, cn_sf_action)
+  int collect;            // CrowdSimVarNumCollect-v0 (cn_env_create_collect): pred_info observation, collect reward / goals
+  double frame_dt;        // config.data.pred_timestep: pred_info's frame = global_time / frame_dt
 };
 
 // Struct-of-arrays environment state in HBM.  Per-human arrays are [N][H] (human index
@@ -123,6 +125,11 @@ struct CnState {
   // overflow ORCA lines (k >= line_cap) of every step-kernel thread: [grid * block][ovf_stride] float4
   void *line_ovf;
   int ovf_stride;
+  // CrowdSimVarNumCollect-v0 only (crowd_sim_var_num_collect.py; null otherwise)
+  int *pred_id;                      // [N][H] human_pred_id
+  int *max_id;                       // [N] max_human_id: the next fresh prediction id
+  uint8_t *rgoal_due;                // [N] ReachGoal this step: the event kernel draws the robot's next goal
+  double *rgoal_med;                 // [N][2] np.median of the humans' positions before the step (that draw's first branch)
 };
 
 // Caller-owned observation/result buffers (PyTorch tensors in the host mirror).
@@ -132,6 +139,7 @@ struct CnObs {
   float *spatial_edges;       // [N,H,W]
   float *detected_human_num;  // [N,1]
   uint8_t *visible_masks;     // [N,H] or nullptr
+  float *pred_info;           // [N,H,4] CrowdSimVarNumCollect-v0 only: frame, prediction id, px, py (inf: not visible)
 };
 
 struct CnStepOut {

@@ -480,6 +480,109 @@ CN_HD void cn_phase_reward(const CnParams& p, const CnState& g, CnEnvSh& s, int 
   g.step_count[e] = step + 1;
 }
 
+// ------------------------------------------------------------------------------------------
+// CrowdSimVarNumCollect-v0 (crowd_sim/envs/crowd_sim_var_num_collect.py): the data-collection environment of
+// collect_data.py.  CrowdSimVarNum.step with its own calc_reward, generate_ob and reset bookkeeping.
+
+// k-th smallest of v[0..n) (counting selection: n <= 128 and it runs only on ReachGoal steps)
+CN_HD double cn_kth_smallest(const double* v, int n, int k) {
+  for (int i = 0; i < n; ++i) {
+    int lt = 0, le = 0;
+    for (int j = 0; j < n; ++j) { lt += v[j] < v[i] ? 1 : 0; le += v[j] <= v[i] ? 1 : 0; }
+    if (lt <= k && k < le) return v[i];
+  }
+  return v[0];
+}
+// np.median(x) of n values: the middle one, or the mean of the two middle ones ((a + b) / 2, np.mean's order)
+CN_HD double cn_median(const double* v, int n) {
+  if (n & 1) return cn_kth_smallest(v, n, n / 2);
+  return (cn_kth_smallest(v, n, n / 2 - 1) + cn_kth_smallest(v, n, n / 2)) / 2.0;
+}
+
+// Phase REWARD of the collect environment (leader; crowd_sim_var_num_collect.py:136-189): reward 0, done only at
+// global_time >= 40000; info Collision (the episode goes on), else ReachGoal, else Nothing.  ReachGoal stores the median
+// of the humans' positions before the step and flags the robot's goal draw, which the event kernel makes on the
+// environment's MT19937 stream ahead of that step's human goal changes (cn_phase_goals<true>).  Then the robot moves.
+CN_HD void cn_collect_reward(const CnParams& p, const CnState& g, CnEnvSh& s, int e, const CnStepOut& out) {
+  const int H = s.hn;
+  bool collision = false;
+  for (int i = 0; i < H; ++i) {
+    const double dx = s.px[i] - s.rpx, dy = s.py[i] - s.rpy;
+    if (sqrt(dx * dx + dy * dy) - s.rad[i] - p.robot_radius < 0) { collision = true; break; }
+  }
+  const bool reaching_goal = cn_norm_dot(s.rpx - s.rgx, s.rpy - s.rgy) < p.robot_radius;
+  const int step = g.step_count[e];
+  int done = 0, info = CN_INFO_NOTHING;
+  bool draw = false;
+  if (step * p.time_step >= 40000.0) { done = 1; info = CN_INFO_TIMEOUT; }
+  else if (collision) info = CN_INFO_COLLISION;
+  else if (reaching_goal) {
+    info = CN_INFO_REACHGOAL;
+    draw = true;
+    g.rgoal_med[2 * e] = cn_median(s.px, H);
+    g.rgoal_med[2 * e + 1] = cn_median(s.py, H);
+  }
+  g.rgoal_due[e] = draw ? 1 : 0;
+  s.reward = 0.0; s.done = done; s.info = info;
+  const int len = g.ep_len[e] + 1;
+  g.ep_len[e] = len;
+  out.reward[e] = 0.0f;
+  out.done[e] = (uint8_t)done;
+  out.info[e] = info;
+  out.info_aux[e] = 0.0f;
+  if (out.not_done) out.not_done[e] = done ? 0.0f : 1.0f;
+  if (done) { out.ep_ret[e] = g.ep_ret[e]; out.ep_len[e] = len; }
+  if (p.robot_policy == 2) {
+    s.rpx = s.rpx + s.nrwx * p.time_step;
+    s.rpy = s.rpy + s.nrwy * p.time_step;
+    s.rwx = s.nrwx; s.rwy = s.nrwy;
+  } else {
+    s.rpx = s.rpx + (double)s.ax * p.time_step;
+    s.rpy = s.rpy + (double)s.ay * p.time_step;
+  }
+  s.rvx = s.ax; s.rvy = s.ay;
+  g.step_count[e] = step + 1;
+}
+
+// set bits of the bit string `m` (32-bit words) in positions [lo, hi)
+CN_HD int cn_mask_count(const uint32_t* m, int lo, int hi) {
+  int c = 0;
+  for (int b = lo; b < hi;) {
+    const int o = b & 31;
+    const int n = (32 - o) < (hi - b) ? (32 - o) : (hi - b);
+    const uint32_t bits = (m[b >> 5] >> o) & (n == 32 ? 0xffffffffu : ((1u << n) - 1u));
+    c += cn_popc(bits);
+    b += n;
+  }
+  return c;
+}
+
+// Prediction ids and the pred_info row of human h (crowd_sim_var_num_collect.py:98-131), after cn_phase_obs_a.
+// `leaving` = bit string over the CTA's threads (bit first + k = human k of this environment): humans the robot saw at
+// the previous observation and does not see now.  They get fresh ids max_human_id, max_human_id + 1, ... in ascending
+// human index, i.e. max_human_id + (leaving humans below h).  At an install (reset_flag) ids restart at arange(hn) and
+// nobody leaves (last_human_observability = zeros).  The row: [global_time / data.pred_timestep, id, px, py] with the
+// belief position of a visible human and inf otherwise.  The leader updates max_id after the caller's next barrier
+// (cn_collect_ids_done): every thread of the environment reads it here first.
+CN_HD void cn_collect_ids(const CnParams& p, const CnState& g, const CnEnvSh& s, int e, int h, const uint32_t* leaving,
+                          int first, const CnObs& ob) {
+  const size_t i = cn_idx(p, e, h);
+  float* row = ob.pred_info + i * 4;
+  if (h >= s.hn) { row[0] = row[1] = row[2] = row[3] = INFINITY; return; }
+  int id = s.reset_flag ? h : g.pred_id[i];
+  if ((leaving[(first + h) >> 5] >> ((first + h) & 31)) & 1u) id = g.max_id[e] + cn_mask_count(leaving, first, first + h);
+  g.pred_id[i] = id;
+  const bool vis = s.visr[h] != 0;
+  row[0] = (float)((g.step_count[e] * p.time_step) / p.frame_dt);
+  row[1] = (float)id;
+  row[2] = vis ? (float)g.bpx[i] : INFINITY;
+  row[3] = vis ? (float)g.bpy[i] : INFINITY;
+}
+CN_HD void cn_collect_ids_done(const CnParams& p, const CnState& g, const CnEnvSh& s, int e, const uint32_t* leaving,
+                               int first) {
+  g.max_id[e] = (s.reset_flag ? s.hn : g.max_id[e]) + cn_mask_count(leaving, first, first + p.H);
+}
+
 // Phase INTEGRATE (per human): humans[i].step(human_action).
 CN_HD void cn_phase_integrate(const CnParams& p, CnEnvSh& s, int h) {
   if (p.social_force) {
@@ -981,10 +1084,26 @@ CN_HD void cn_phase_obs_c(const CnParams& p, CnEnvSh& s, int e, int h, const CnO
 // (crowd_sim_pred.py:202-211).  Replicated execution over the lanes of `co` (see CnCoop): every lane
 // draws the same random numbers from `key`; collision scans are lane-strided; lane 0 owns the writes.
 // Returns true when a search exhausted `budget` tries (see cn_prepare_env): the caller must NOT store the working set.
+// COLLECT (CrowdSimVarNumCollect-v0): first the robot's new goal after a ReachGoal (crowd_sim_var_num_collect.py:172-184,
+// inside calc_reward, so ahead of every draw of the humans' goal changes and respawns): with probability 0.5 the median
+// of the humans' positions before the step, else a uniform point of the arena.
+template <bool COLLECT = false>
 CN_HD bool cn_phase_goals(const CnParams& p, const CnState& g, CnEnvSh& s, int e, uint32_t* key, const CnCoop& co,
                           int budget = 0) {
   const int H = s.hn;           // live humans
   CnRng rng; rng.key = key; rng.pos = g.mt_pos[e]; rng.budget = budget; rng.deferred = 0;
+  if (COLLECT && g.rgoal_due[e]) {
+    double gx, gy;
+    if (cn_rng_double(rng, co) < 0.5) {                         // np.random.uniform(0, 1) < 0.5
+      gx = g.rgoal_med[2 * e]; gy = g.rgoal_med[2 * e + 1];
+    } else {                                                    // np.random.uniform(-arena, arena, size=2)
+      gx = cn_rng_uniform(rng, co, -p.arena_size, p.arena_size);
+      gy = cn_rng_uniform(rng, co, -p.arena_size, p.arena_size);
+    }
+    cn_coop_sync(co);
+    if (co.lane == 0) { s.rgx = gx; s.rgy = gy; }
+    cn_coop_sync(co);
+  }
   double nd = g.nd_global[e];
   const int step = g.step_count[e];
   // global_time % 5 == 0 with global_time = step * 0.25 accumulated exactly

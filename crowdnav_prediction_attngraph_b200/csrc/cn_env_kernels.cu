@@ -69,7 +69,9 @@ __device__ inline CnEnvSh* env_view(unsigned char* base, const EnvSmemLayout& L,
 // the same launch.  mode 1 = reset of the whole vector env: no step, every environment installs.
 // ROBOT: robot_policy != 0 (the robot's ORCA / social-force solve, cn_robot_act); a separate instantiation so the network
 // policy's kernel carries none of its code.  VIS: robot_visible != 0 (the humans' solves see the robot), likewise.
-template <int MAXH, int MAXW, bool ROBOT, bool VIS>
+// COLLECT: CrowdSimVarNumCollect-v0 (p.collect): collect reward, prediction ids and the pred_info rows instead of the
+// training observation.  Phase 'train' only (cn_env_create_collect), so it carries no ground-truth look-ahead.
+template <int MAXH, int MAXW, bool ROBOT, bool VIS, bool COLLECT = false>
 __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState g, const float* __restrict__ action,
                                                           CnObs ob, CnStepOut out, int epb, int line_cap, int mode) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -190,7 +192,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
       if (active && h == 0) g.lp_cost[e] = s->lp3_cost;
       return;
     }
-    if (p.test_phase) {
+    if (p.test_phase && !COLLECT) {
       // phase 'test': ground-truth look-ahead (crowd_sim_pred.py:136-138 -> crowd_sim_var_num.py:180-206):
       // lookahead_steps nested solves on a scratch copy of the joint state kept in the same shared arrays
       // (every thread saves / restores its own human), then the 'future' danger zone inputs for the reward.
@@ -230,7 +232,11 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
     }
   }
   __syncthreads();
-  if (mode != 1 && active && h == 0) cn_phase_reward(p, g, *s, e, out);
+  if (mode != 1 && active && h == 0) {
+    if (COLLECT) cn_collect_reward(p, g, *s, e, out);
+    else cn_phase_reward(p, g, *s, e, out);
+  }
+  if (COLLECT && mode == 1 && active && h == 0) g.rgoal_due[e] = 0;
   __syncthreads();
   if (active) {
     if (s->done) cn_install_env(p, g, *s, e, h);      // finished: the prepared next episode takes over
@@ -242,6 +248,29 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
     __syncthreads();
   }
   float row[MAXW];
+  if (COLLECT) {
+    // generate_ob of the collect environment: visibility and belief as usual (cn_phase_obs_a), then the prediction ids
+    // of the humans that left the robot's view, numbered in ascending human index across the environment's threads
+    // (which may span two warps): one ballot per warp, prefix popcounts over the CTA's bit string
+    __shared__ uint32_t leaving[(288 + 31) / 32];
+    const bool seen_before = active && h < s->hn && g.vis[cn_idx(p, e, h)] != 0;
+    if (active) cn_phase_obs_a<MAXW>(p, g, *s, e, h, row);
+    __syncthreads();
+    const uint32_t b = __ballot_sync(0xffffffffu, seen_before && !s->reset_flag && !s->visr[h]);
+    if (lane == 0) leaving[warp] = b;
+    __syncthreads();
+    if (active) cn_collect_ids(p, g, *s, e, h, leaving, le * H, ob);
+    __syncthreads();
+    if (active) cn_phase_store(p, g, *s, e, h);
+    if (active && h == 0) {
+      cn_collect_ids_done(p, g, *s, e, leaving, le * H);
+      int evt = cn_event_flag(p, g, *s, e);
+      if (evt == 0 && g.rgoal_due[e]) evt = 1;                        // the robot's goal draw (cn_phase_goals<true>)
+      g.evt[e] = (uint8_t)evt;
+      if (mode != 2) g.lp_cost[e] = s->lp3_cost;
+    }
+    return;
+  }
   if (active) cn_phase_obs_a<MAXW>(p, g, *s, e, h, row);
   __syncthreads();
   if (active) cn_phase_obs_b(p, g, *s, e, h, row, ob);
@@ -263,7 +292,9 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
 // lane-strided.  Nothing here touches observation buffers, so the kernel runs on the engine's side
 // stream, overlapped with the policy; the next step kernel waits for it.  Warps whose environment has
 // no event (g.evt == 0) exit immediately.
+// COLLECT: the collect environment's instantiation, whose goal dynamics start with the robot's goal draw.
 #define CN_EVENT_WARPS 4
+template <bool COLLECT = false>
 __global__ void __launch_bounds__(CN_EVENT_WARPS * 32) cn_env_event_kernel(CnParams p, CnState g, int force,
                                                                            size_t per_warp_bytes) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -291,7 +322,7 @@ __global__ void __launch_bounds__(CN_EVENT_WARPS * 32) cn_env_event_kernel(CnPar
     for (int h = lane; h < H; h += 32) cn_phase_load(p, g, *s, e, h, nullptr);
     for (int i = lane; i < 624; i += 32) key[i] = g.mt[(size_t)e * 624 + i];
     __syncwarp();
-    deferred = cn_phase_goals(p, g, *s, e, key, co, p.defer_tries);
+    deferred = cn_phase_goals<COLLECT>(p, g, *s, e, key, co, p.defer_tries);
     __syncwarp();
     if (!deferred) {
       for (int h = lane; h < H; h += 32) cn_phase_store(p, g, *s, e, h);
@@ -315,6 +346,7 @@ __global__ void __launch_bounds__(CN_EVENT_WARPS * 32) cn_env_event_kernel(CnPar
 // scope: the MT19937 twist runs 224 words at a time and the <= 104 candidates up to the next twist are evaluated at
 // once, CN_HEAVY_SUB threads per candidate splitting the agent list.  Results are identical to the sequential loop
 // (first free candidate, same stream position).
+template <bool COLLECT = false>
 __global__ void __launch_bounds__(CN_HEAVY_THREADS) cn_env_event_heavy_kernel(CnParams p, CnState g) {
   extern __shared__ __align__(16) unsigned char smem[];
   const int H = p.H;
@@ -339,7 +371,7 @@ __global__ void __launch_bounds__(CN_HEAVY_THREADS) cn_env_event_heavy_kernel(Cn
       for (int h = threadIdx.x; h < H; h += blockDim.x) cn_phase_load(p, g, *s, e, h, nullptr);
       for (int i = threadIdx.x; i < 624; i += blockDim.x) key[i] = g.mt[(size_t)e * 624 + i];
       __syncthreads();
-      cn_phase_goals(p, g, *s, e, key, co, 0);
+      cn_phase_goals<COLLECT>(p, g, *s, e, key, co, 0);
       __syncthreads();
       for (int h = threadIdx.x; h < H; h += blockDim.x) cn_phase_store(p, g, *s, e, h);
       for (int i = threadIdx.x; i < 624; i += blockDim.x) g.mt[(size_t)e * 624 + i] = key[i];
@@ -476,7 +508,15 @@ KernelFn pick_kernel_vis(int maxh, bool robot) {
   return cn_env_step_kernel<128, 16, false, VIS>;
 }
 
-KernelFn pick_kernel(int maxh, bool robot, bool vis) {
+// the collect environment: robot policy and visibility stay run-time parameters there (it runs no network policy)
+KernelFn pick_kernel_collect(int maxh) {
+  if (maxh <= 32) return cn_env_step_kernel<32, 16, true, true, true>;
+  if (maxh <= 64) return cn_env_step_kernel<64, 16, true, true, true>;
+  return cn_env_step_kernel<128, 16, true, true, true>;
+}
+
+KernelFn pick_kernel(int maxh, bool robot, bool vis, bool collect = false) {
+  if (collect) return pick_kernel_collect(maxh);
   return vis ? pick_kernel_vis<true>(maxh, robot) : pick_kernel_vis<false>(maxh, robot);
 }
 
@@ -484,18 +524,26 @@ CnObs to_obs(const cn_obs_ptrs* o) {
   CnObs ob;
   ob.robot_node = o->robot_node; ob.temporal_edges = o->temporal_edges; ob.spatial_edges = o->spatial_edges;
   ob.detected_human_num = o->detected_human_num; ob.visible_masks = o->visible_masks;
+  ob.pred_info = nullptr;
   return ob;
 }
 
 int event_kernel(cn_env* env, int force, cudaStream_t stream) {
   const int grid = (env->p.N + CN_EVENT_WARPS - 1) / CN_EVENT_WARPS;
-  cn_env_event_kernel<<<grid, CN_EVENT_WARPS * 32, CN_EVENT_WARPS * env->reset_warp_bytes, stream>>>(
-      env->p, env->g, force, env->reset_warp_bytes);
+  if (env->p.collect)
+    cn_env_event_kernel<true><<<grid, CN_EVENT_WARPS * 32, CN_EVENT_WARPS * env->reset_warp_bytes, stream>>>(
+        env->p, env->g, force, env->reset_warp_bytes);
+  else
+    cn_env_event_kernel<<<grid, CN_EVENT_WARPS * 32, CN_EVENT_WARPS * env->reset_warp_bytes, stream>>>(
+        env->p, env->g, force, env->reset_warp_bytes);
   env->launches += 1;
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return cn_set_error("cn_env_event_kernel launch: %s", cudaGetErrorString(err));
   // deferred (pathological) searches, one CTA each; an empty list costs one ~2 us launch on the side stream
-  cn_env_event_heavy_kernel<<<env->heavy_grid, CN_HEAVY_THREADS, env->heavy_smem, stream>>>(env->p, env->g);
+  if (env->p.collect)
+    cn_env_event_heavy_kernel<true><<<env->heavy_grid, CN_HEAVY_THREADS, env->heavy_smem, stream>>>(env->p, env->g);
+  else
+    cn_env_event_heavy_kernel<<<env->heavy_grid, CN_HEAVY_THREADS, env->heavy_smem, stream>>>(env->p, env->g);
   env->launches += 1;
   err = cudaGetLastError();
   if (err != cudaSuccess) return cn_set_error("cn_env_event_heavy_kernel launch: %s", cudaGetErrorString(err));
@@ -514,7 +562,7 @@ int join_side(cn_env* env, cudaStream_t stream) {
 // step (or mode 1: install-everything) kernel on the caller's stream, then the event kernel behind it
 // on the side stream
 int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const cn_step_ptrs* r, int mode,
-                cudaStream_t stream) {
+                cudaStream_t stream, float* d_pred_info = nullptr) {
   CnStepOut out;
   memset(&out, 0, sizeof(out));
   if (r) {
@@ -530,13 +578,14 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
     env->prep_dirty = false;
   }
   const int grid = (env->p.N + env->epb - 1) / env->epb;
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0, env->p.collect != 0);
+  CnObs ob = to_obs(o);
+  ob.pred_info = d_pred_info;
   // mode 0 with a pre-solve of this state done on the side stream (joined above) -> finishing pass only (mode 2)
   const int kmode = (mode == 0 && env->presolved) ? 2 : mode;
   env->presolved = false;
   if (env->profile) cudaEventRecord(env->pev[0], stream);
-  fn<<<grid, env->threads, env->smem_bytes, stream>>>(env->p, env->g, d_action, to_obs(o), out, env->epb, env->line_cap,
-                                                      kmode);
+  fn<<<grid, env->threads, env->smem_bytes, stream>>>(env->p, env->g, d_action, ob, out, env->epb, env->line_cap, kmode);
   if (env->profile) cudaEventRecord(env->pev[1], stream);
   env->launches += 1;
   cudaError_t err = cudaGetLastError();
@@ -559,7 +608,7 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
     // visible it also reads the robot's position and velocity, and both are final once this step has integrated (the
     // next action moves the robot only after the humans' solve).  It runs here, on the side stream, while the caller's
     // stream runs the policy; the next step only finishes (robot move, reward, integration, observation).
-    fn<<<grid, env->threads, env->smem_bytes, env->side>>>(env->p, env->g, nullptr, to_obs(o), out, env->epb, env->line_cap, 3);
+    fn<<<grid, env->threads, env->smem_bytes, env->side>>>(env->p, env->g, nullptr, ob, out, env->epb, env->line_cap, 3);
     env->launches += 1;
     err = cudaGetLastError();
     if (err != cudaSuccess) return cn_set_error("cn_env_step_kernel (pre-solve) launch: %s", cudaGetErrorString(err));
@@ -578,7 +627,11 @@ extern "C" {
 
 int cn_abi_version(void) { return CN_ABI_VERSION; }
 
-int cn_env_create(const cn_config* cfg, cn_env** out) {
+}  // extern "C"
+
+namespace {
+
+int env_create(const cn_config* cfg, cn_env** out, bool collect) {
   if (!cfg || !out) return cn_set_error("cn_env_create: null argument");
   *out = nullptr;
   if (cfg->num_envs <= 0 || cfg->human_num <= 0 || cfg->human_num_range < 0 || cfg->human_num_range >= cfg->human_num ||
@@ -691,6 +744,8 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   p.sf_A = cfg->sf_A; p.sf_B = cfg->sf_B; p.sf_KI = cfg->sf_KI;
   p.robot_policy = cfg->robot_policy;
   p.robot_visible = cfg->robot_visible;
+  p.collect = collect ? 1 : 0;
+  p.frame_dt = cfg->pred_timestep;
   {
     // warp-scope budget of rejection-sampling tries before an event goes to the CTA-scope kernel
     // (CN_DEFER_TRIES=1 sends every search that needs a second candidate there: parity tests of the heavy path)
@@ -719,6 +774,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   A(hwx, cfg->human_policy ? NH : (size_t)4); A(hwy, cfg->human_policy ? NH : (size_t)4);
   A(rwx, cfg->robot_policy == 2 ? N : (size_t)4); A(rwy, cfg->robot_policy == 2 ? N : (size_t)4);
   A(rsim_exists, N); A(rsim_nd, N); A(rsim_rother, cfg->robot_policy == 1 ? NH : (size_t)4);
+  if (collect) { A(pred_id, NH); A(max_id, N); A(rgoal_due, N); A(rgoal_med, 2 * N); }
 #undef A
   if (!rc) {
     // nd_global starts at the configured value (config.orca.neighbor_dist)
@@ -758,8 +814,16 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   const EnvSmemLayout L = env_layout(p.H, true, p.social_force != 0);
   int nsm = 0;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0);
-  err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0, collect);
+  // dynamic shared memory: 227 KiB less the kernel's static part (the collect instantiation's ballot words)
+  size_t smem_cap = 227 * 1024;
+  {
+    cudaFuncAttributes fa;
+    err = cudaFuncGetAttributes(&fa, fn);
+    if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncGetAttributes: %s", cudaGetErrorString(err)); }
+    smem_cap -= fa.sharedSizeBytes;
+  }
+  err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cap);
   if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncSetAttribute: %s", cudaGetErrorString(err)); }
   // ORCA lines per human: one per other human, plus one for the robot when it is visible
   const int max_lines = p.H - 1 + p.robot_visible;
@@ -775,7 +839,7 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
       const size_t need = align16((size_t)epb * L.per_env) + (size_t)cap * epb * p.H * sizeof(float4) +
                           (size_t)(threads / 16) * p.H * sizeof(float4) +         // + per-half-warp LP3 scratch
                           align16(8 + 2 * (size_t)threads);                       // + CTA LP3 task queue
-      if (need > 227 * 1024) continue;
+      if (need > smem_cap) continue;
       int per_sm = 0;
       err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, need);
       if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("occupancy query: %s", cudaGetErrorString(err)); }
@@ -815,8 +879,10 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
   }
   // event kernel: per-warp working set + MT19937 state
   env->reset_warp_bytes = align16(env_layout(p.H, false, p.social_force != 0).per_env + 624 * sizeof(uint32_t) + 5 * CN_FTAB * sizeof(float));
-  err = cudaFuncSetAttribute(cn_env_event_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(CN_EVENT_WARPS * env->reset_warp_bytes));
+  err = collect ? cudaFuncSetAttribute(cn_env_event_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(CN_EVENT_WARPS * env->reset_warp_bytes))
+                : cudaFuncSetAttribute(cn_env_event_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(CN_EVENT_WARPS * env->reset_warp_bytes));
   if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncSetAttribute(reset): %s", cudaGetErrorString(err)); }
   // heavy path: working set + MT19937 state + a few ints of scratch per CTA; half an SM-wave of CTAs (the list
   // is short, and these CTAs share the GPU with the caller's policy kernels)
@@ -827,10 +893,50 @@ int cn_env_create(const cn_config* cfg, cn_env** out) {
     env->heavy_grid = sms / 2 > 0 ? sms / 2 : 1;
     if (env->heavy_grid > p.N) env->heavy_grid = p.N;
   }
-  err = cudaFuncSetAttribute(cn_env_event_heavy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)env->heavy_smem);
+  err = collect ? cudaFuncSetAttribute(cn_env_event_heavy_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)env->heavy_smem)
+                : cudaFuncSetAttribute(cn_env_event_heavy_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)env->heavy_smem);
   if (err != cudaSuccess) { cn_env_destroy(env); return cn_set_error("cudaFuncSetAttribute(heavy): %s", cudaGetErrorString(err)); }
   *out = env;
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cn_env_create(const cn_config* cfg, cn_env** out) { return env_create(cfg, out, false); }
+
+int cn_env_create_collect(const cn_config* cfg, cn_env** out) {
+  if (!cfg || !out) return cn_set_error("cn_env_create_collect: null argument");
+  *out = nullptr;
+  if (cfg->const_vel)
+    return cn_set_error("cn_env_create_collect: CrowdSimVarNumCollect-v0 subclasses CrowdSimVarNum-v0 (const_vel 0)");
+  if (cfg->human_num_range > 0)
+    return cn_set_error("cn_env_create_collect: human_num_range > 0 is not covered: the reference raises there "
+                        "(crowd_sim_var_num_collect.py:121-123 joins human_num frame rows with human_num + range position rows)");
+  if (cfg->phase != 0)
+    return cn_set_error("cn_env_create_collect: phase 'test' is not covered: the reference raises on the first step (the "
+                        "ground-truth look-ahead reads self.human_visibility, crowd_sim_var_num.py:225, which the collect "
+                        "environment's generate_ob never sets)");
+  return env_create(cfg, out, true);
+}
+
+int cn_env_reset_collect(cn_env* env, float* d_pred_info, void* stream) {
+  if (!env || !d_pred_info) return cn_set_error("cn_env_reset_collect: null argument");
+  if (!env->p.collect) return cn_set_error("cn_env_reset_collect: the handle was not made by cn_env_create_collect");
+  CnDeviceGuard guard(env->device);
+  return launch_step(env, nullptr, &env->d_obs, nullptr, 1, (cudaStream_t)stream, d_pred_info);
+}
+
+int cn_env_step_collect(cn_env* env, const float* d_action, float* d_pred_info, const cn_step_ptrs* d_out, void* stream) {
+  if (!env || !d_action || !d_pred_info || !d_out) return cn_set_error("cn_env_step_collect: null argument");
+  if (!env->p.collect) return cn_set_error("cn_env_step_collect: the handle was not made by cn_env_create_collect");
+  if (!d_out->reward || !d_out->done || !d_out->info || !d_out->info_aux || !d_out->ep_ret || !d_out->ep_len)
+    return cn_set_error("cn_env_step_collect: every cn_step_ptrs field must be set");
+  CnDeviceGuard guard(env->device);
+  return launch_step(env, d_action, &env->d_obs, d_out, 0, (cudaStream_t)stream, d_pred_info);
 }
 
 int cn_env_destroy(cn_env* env) {
@@ -848,6 +954,7 @@ int cn_env_destroy(cn_env* env) {
 
 int cn_env_reset(cn_env* env, const cn_obs_ptrs* d_obs, void* stream) {
   if (!env || !d_obs) return cn_set_error("cn_env_reset: null argument");
+  if (env->p.collect) return cn_set_error("cn_env_reset: a collect environment resets with cn_env_reset_collect");
   CnDeviceGuard guard(env->device);
   // a reset of the whole vec env restarts Monitor bookkeeping but NOT case_counter (it keeps advancing)
   return launch_step(env, nullptr, d_obs, nullptr, 1, (cudaStream_t)stream);
@@ -856,6 +963,7 @@ int cn_env_reset(cn_env* env, const cn_obs_ptrs* d_obs, void* stream) {
 int cn_env_step(cn_env* env, const float* d_action, const cn_obs_ptrs* d_obs, const cn_step_ptrs* d_out,
                 void* stream) {
   if (!env || !d_action || !d_obs || !d_out) return cn_set_error("cn_env_step: null argument");
+  if (env->p.collect) return cn_set_error("cn_env_step: a collect environment steps with cn_env_step_collect");
   if (!d_out->reward || !d_out->done || !d_out->info || !d_out->info_aux || !d_out->ep_ret || !d_out->ep_len)
     return cn_set_error("cn_env_step: every cn_step_ptrs field must be set");
   CnDeviceGuard guard(env->device);
@@ -864,6 +972,7 @@ int cn_env_step(cn_env* env, const float* d_action, const cn_obs_ptrs* d_obs, co
 
 int cn_env_step_host(cn_env* env, const float* h_action, const cn_obs_ptrs* h_obs, const cn_step_ptrs* h_out) {
   if (!env || !h_action || !h_obs || !h_out) return cn_set_error("cn_env_step_host: null argument");
+  if (env->p.collect) return cn_set_error("cn_env_step_host: a collect environment steps with cn_env_step_collect");
   cudaSetDevice(env->device);
   const size_t N = (size_t)env->p.N, NH = N * env->p.H;
   cudaStream_t st = 0;

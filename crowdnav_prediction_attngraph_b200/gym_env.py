@@ -152,3 +152,37 @@ class CrowdSimPredRealGST(_GymCrowdEnv):
     """crowd_sim/envs/crowd_sim_pred_real_gst.py: the raw (unsorted, 2-wide) observation the GST wrapper consumes."""
     _engine_id = "CrowdSimVarNum-v0"
     _unsorted = True
+
+
+class CrowdSimVarNumCollect(_GymCrowdEnv):
+    """crowd_sim/envs/crowd_sim_var_num_collect.py: the data-collection environment of collect_data.py, observation
+    {'pred_info': [H, 4]} (frame, prediction id, px, py; inf where the robot does not see the human)."""
+    _engine_id = "CrowdSimVarNumCollect-v0"
+
+    def configure(self, config):
+        super().configure(config)
+        H = config.sim.human_num + config.sim.human_num_range
+        self.observation_space = _DictSpace({'pred_info': Box((H, 4))})
+
+    def _build(self):
+        from .collect import CudaCollectVecEnv
+        if self.config is None:
+            raise AttributeError('robot has to be set!')
+        if self.thisSeed is None or self.nenv is None:
+            raise AttributeError("env.thisSeed and env.nenv must be set before reset() (rl/networks/envs.py:51-58)")
+        phase = self.phase if self.phase is not None else 'train'
+        d = config_dict_from_reference(self.config, 1, int(self.thisSeed), self._engine_id, nenv_total=int(self.nenv),
+                                       rank_offset=0, device_index=self._device.index or 0, phase=phase)
+        self._venv = CudaCollectVecEnv(device=self._device, cfg=d)
+
+    def reset(self, phase='train', test_case=None):
+        if self._venv is None:
+            self._build()
+        return {'pred_info': self._venv.reset_device()[0].cpu().numpy()}
+
+    def step(self, action, update=True):
+        if self._venv is None:
+            raise RuntimeError("step() before reset()")
+        a = torch.from_numpy(np.asarray(action, dtype=np.float32).reshape(1, 2).copy()).to(self._device)
+        obs, _, done, infos = self._venv.step(a)
+        return {'pred_info': obs['pred_info'][0]}, 0, bool(done[0]), {'info': infos[0]['info']}

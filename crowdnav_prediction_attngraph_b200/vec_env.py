@@ -83,6 +83,28 @@ class Box(_Space):
 
 # robot.policy -> cn_config.robot_policy (0: the caller's action)
 ROBOT_POLICIES = {"orca": 1, "social_force": 2}
+COLLECT_ENV = "CrowdSimVarNumCollect-v0"
+
+
+def _check_collect(config, seed, phase, nenv_total):
+    """The collect environment's limits.  Returns `seed` as the int32 with the same 32 bits (cn_config.seed)."""
+    if int(config.sim.human_num_range) > 0:
+        raise NotImplementedError(
+            "CrowdSimVarNumCollect-v0 with sim.human_num_range > 0 is not covered: the reference raises there "
+            "(crowd_sim_var_num_collect.py:121-123 concatenates human_num frame rows with human_num + range position rows)")
+    if phase == "test":
+        raise NotImplementedError(
+            "CrowdSimVarNumCollect-v0 in phase 'test' (one environment, config.data.render) is not covered: the reference "
+            "raises on its first step (the ground-truth look-ahead reads self.human_visibility, crowd_sim_var_num.py:225, "
+            "which the collect environment's generate_ob never sets)")
+    seed = int(seed)
+    if not 0 <= seed < 2 ** 32:
+        raise ValueError("seed %d: the collect environment takes seeds in [0, 2**32)" % seed)
+    top = 2000 + seed + nenv_total - 1          # np.random.seed(counter_offset['train'] + case_counter + seed + rank)
+    if top >= 2 ** 32:
+        raise ValueError("seed %d: the reference's np.random.seed(2000 + seed + rank) gets %d >= 2**32 and raises "
+                         "(crowd_sim.py:386-387)" % (seed, top))
+    return seed - 2 ** 32 if seed >= 2 ** 31 else seed
 
 
 def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None, rank_offset=0, device_index=0,
@@ -101,7 +123,7 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         if config.sim.predict_method != "const_vel":
             raise NotImplementedError("CrowdSimPred-v0 is covered for predict_method='const_vel'")
         const_vel = 1
-    elif env_name == "CrowdSimVarNum-v0":
+    elif env_name in ("CrowdSimVarNum-v0", COLLECT_ENV):
         const_vel = 0
     else:
         raise NotImplementedError("env id %r is not covered by the CUDA engine" % env_name)
@@ -123,6 +145,9 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
         if int(config.sim.human_num_range) > 0:
             raise NotImplementedError("robot.policy %r with sim.human_num_range > 0 is not covered (the robot's rvo2 "
                                       "simulator would be rebuilt as humans join and leave)" % (config.robot.policy,))
+    if env_name == COLLECT_ENV:
+        seed = _check_collect(config, seed, phase, nenv_total or num_envs)
+        allow_unsorted = True           # the collect observation is never sorted
     sort_humans = getattr(getattr(config, "args", None), "sort_humans", True)
     if not sort_humans and not allow_unsorted:
         # the policy mirror masks attention with detected_human_num, which is only valid for distance-sorted rows
@@ -441,6 +466,9 @@ def make_vec_envs(env_name, seed, num_processes, gamma, log_dir, device, allow_e
     d = config_dict_from_reference(config, num_processes, seed, env_name, nenv_total=nenv_total,
                                    rank_offset=rank_offset,
                                    device_index=device.index if device.index is not None else 0, phase=phase)
+    if env_name == COLLECT_ENV:
+        from .collect import CudaCollectVecEnv
+        return CudaCollectVecEnv(device=device, cfg=d, wrap_pytorch=wrap_pytorch)
     return CudaCrowdVecEnv(device=device, cfg=d)
 
 

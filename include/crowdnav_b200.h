@@ -171,6 +171,42 @@ int cn_env_profile(cn_env *env, int enable);
 int cn_env_stage_ms(cn_env *env, float *out3);
 
 /* ------------------------------------------------------------------------------------------ */
+/* Data collection: CrowdSimVarNumCollect-v0 (crowd_sim/envs/crowd_sim_var_num_collect.py), the environment collect_data.py
+ * steps to build the GST predictor's training set.  CrowdSimVarNum-v0's step (robot_policy, robot_visible, human_policy
+ * and phase as in cn_env_create) with the collect environment's own parts: reward 0; done only at global_time >= 40000;
+ * info Collision (the episode goes on), ReachGoal (the robot draws a new goal on the environment's legacy numpy stream:
+ * the median of the humans' positions or a uniform point of the arena) or Nothing; the observation pred_info [N,H,4]
+ * float32, one row per human: [global_time / pred_timestep, prediction id, px, py] with the belief position of a visible
+ * human and inf otherwise.  Prediction ids start at arange(H) and a human that leaves the robot's view gets the next fresh
+ * id.  human_num_range must be 0 and phase 0 'train' (the reference raises otherwise).  The state fields "pred_id" [N,H] int32, "max_id" [N]
+ * int32 (max_human_id), "rgoal_due" [N] uint8 and "rgoal_med" [N,2] float64 are readable through cn_env_state_copy, the
+ * robot's goal through "rgx" / "rgy".  A collect handle is stepped only by the entry points below.                    */
+int cn_env_create_collect(const cn_config *cfg, cn_env **out);
+int cn_env_reset_collect(cn_env *env, float *d_pred_info, void *stream);
+/* d_action [N,2] float32: the robot's velocity when robot_policy is 0, ignored otherwise (collect_data.py passes zeros
+ * and robot.policy 'orca').  d_out: every field but not_done must be set; reward is 0, ep_ret 0.                      */
+int cn_env_step_collect(cn_env *env, const float *d_action, float *d_pred_info, const cn_step_ptrs *d_out, void *stream);
+
+/* Bulk recorder of pred_info observations (collect_data.py:54-62 for N environments at once).  Each append copies one
+ * observation [N,H,4] into a device chunk of chunk_frames frames; a flush compacts the chunk's visible rows (finite py)
+ * over all environments with a device prefix sum and copies only them to h_rows [n_rows,4] float32, ordered by
+ * environment, then frame, then human index, with h_env_rows [N] rows per environment.  One stream synchronisation per
+ * flush, none per append.  h_rows must hold N * H * chunk_frames rows.                                               */
+typedef struct cn_recorder cn_recorder;
+int cn_recorder_create(int num_envs, int human_num, int chunk_frames, int device, cn_recorder **out);
+int cn_recorder_destroy(cn_recorder *r);
+int cn_recorder_append(cn_recorder *r, const float *d_pred_info, void *stream);
+int cn_recorder_pending(cn_recorder *r);
+int cn_recorder_flush(cn_recorder *r, float *h_rows, int64_t *h_env_rows, int64_t *n_rows, void *stream);
+/* Host text writer: rows of environment e (consecutive in h_rows, h_env_rows[e] of them) go to <dir>/<env_base + e>.txt,
+ * truncated first unless `append`, as collect_data.py writes them: str(frame) \t str(id) \t str(px) \t str(py) \n
+ * with Python's float repr.  cn_format_rows formats n rows into out (cap bytes) and returns the length in bytes (out
+ * untouched when it does not fit).                                                                                  */
+int cn_write_rows_txt(const char *dir, const float *h_rows, const int64_t *h_env_rows, int num_envs, int env_base,
+                      int append);
+int64_t cn_format_rows(const float *h_rows, int64_t n, char *out, int64_t cap);
+
+/* ------------------------------------------------------------------------------------------ */
 /* Attention-graph policy (rl/networks/model.py:56-80, selfAttn_srnn_temp_node.py:360-449).    */
 
 typedef struct cn_policy cn_policy;
