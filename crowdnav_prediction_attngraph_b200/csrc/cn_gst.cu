@@ -57,17 +57,21 @@ __device__ __forceinline__ void gt_ln(float a0, float a1, const float* g, const 
 
 __device__ __forceinline__ float gt_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// process_obs_rew tail: one CTA (32 threads) per environment
-__global__ void __launch_bounds__(32) gt_final_kernel(int N, int H, int P, float thr, float collision_penalty,
-                                                      const float* __restrict__ robot, const float* __restrict__ sp2,
-                                                      const float* __restrict__ fp, const float* __restrict__ pred,
-                                                      float* __restrict__ reward, float* __restrict__ penalty_out,
-                                                      float* __restrict__ out_sp) {
+#define GT_MAXH 128   // humans per environment (max_human_num), as in the environment and the policy
+
+// process_obs_rew tail: one CTA per environment, one thread per human (32 * ceil(H / 32) threads).  The distance keys
+// are computed once into shared memory; a row's rank counts the closer rows and the equally close rows of lower index.
+__global__ void __launch_bounds__(GT_MAXH) gt_final_kernel(int N, int H, int P, float thr, float collision_penalty,
+                                                           const float* __restrict__ robot, const float* __restrict__ sp2,
+                                                           const float* __restrict__ fp, const float* __restrict__ pred,
+                                                           float* __restrict__ reward, float* __restrict__ penalty_out,
+                                                           float* __restrict__ out_sp) {
   cn_pdl_prologue();
-  const int e = blockIdx.x;
+  __shared__ float skey[GT_MAXH], spen[GT_MAXH / 32];
+  const int e = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   const float rx = robot[e * 7], ry = robot[e * 7 + 1];
   float pen = 0.0f;
-  for (int i = threadIdx.x; i < H * GT_T; i += 32) {
+  for (int i = threadIdx.x; i < H * GT_T; i += blockDim.x) {
     const int n = i / GT_T, k = i - n * GT_T;
     if (k < P && fp[(size_t)e * H + n] != 0.0f) {
       const float dx = pred[((size_t)e * H * GT_T + i) * 2] - rx, dy = pred[((size_t)e * H * GT_T + i) * 2 + 1] - ry;
@@ -76,18 +80,24 @@ __global__ void __launch_bounds__(32) gt_final_kernel(int N, int H, int P, float
   }
 #pragma unroll
   for (int o = 16; o; o >>= 1) pen = fminf(pen, __shfl_xor_sync(0xffffffffu, pen, o));
+  if (lane == 0) spen[warp] = pen;
+  for (int n = threadIdx.x; n < H; n += blockDim.x) {
+    const float cx = sp2[((size_t)e * H + n) * 2], cy = sp2[((size_t)e * H + n) * 2 + 1];
+    skey[n] = sqrtf(cx * cx + cy * cy);
+  }
+  __syncthreads();
   if (threadIdx.x == 0) {
+    for (int w = 1; w < nw; ++w) pen = fminf(pen, spen[w]);
     if (reward) reward[e] += pen;
     if (penalty_out) penalty_out[e] = pen;
   }
   const int W = 2 * (P + 1);
-  for (int n = threadIdx.x; n < H; n += 32) {
+  for (int n = threadIdx.x; n < H; n += blockDim.x) {
     const float cx = sp2[((size_t)e * H + n) * 2], cy = sp2[((size_t)e * H + n) * 2 + 1];
-    const float key = sqrtf(cx * cx + cy * cy);
+    const float key = skey[n];
     int rank = 0;
     for (int j = 0; j < H; ++j) {
-      const float ox = sp2[((size_t)e * H + j) * 2], oy = sp2[((size_t)e * H + j) * 2 + 1];
-      const float kj = sqrtf(ox * ox + oy * oy);
+      const float kj = skey[j];
       rank += (kj < key || (kj == key && j < n)) ? 1 : 0;
     }
     float* dst = out_sp + ((size_t)e * H + rank) * W;
@@ -114,11 +124,12 @@ __global__ void __launch_bounds__(32) gt_final_kernel(int N, int H, int P, float
 // The only place masked rows enter a valid row's arithmetic is the soft-max denominator (soft-max over ALL H neighbours,
 // then mask and renormalise, mha.py:236-242): all masked keys share the key vector b_k, so their H - n terms are
 // (H - n) * exp(q . b_k - max).  Results equal a computation over every row up to the order of that sum (~1e-9
-// relative).  gtc_attn_kernel stages the Q|K|V rows of one group in shared memory: at most GT_MAXH humans.
-#define GT_MAXH 32
+// relative).  gtc_attn_kernel stages the Q|K|V rows of one group in dynamic shared memory: H * 768 bytes, 96 KB at
+// GT_MAXH = 128 humans.
 #define GTC_WARPS 8
 
-// one warp per (env, frame) group, lane = human: masks, masked input displacement, group counts, newest-frame bookkeeping
+// one warp per (env, frame) group, humans in chunks of 32 (lane = human - n0): masks, masked input displacement, group
+// counts, newest-frame bookkeeping
 __global__ void __launch_bounds__(GTC_WARPS * 32) gtc_prep_kernel(int N, int H, float* __restrict__ ring_pos, uint8_t* __restrict__ ring_mask,
                                                                    int newest, const float* __restrict__ robot, const float* __restrict__ sp2,
                                                                    const uint8_t* __restrict__ vis, float* __restrict__ rowm,
@@ -129,50 +140,56 @@ __global__ void __launch_bounds__(GTC_WARPS * 32) gtc_prep_kernel(int N, int H, 
   const int lane = threadIdx.x & 31;
   const int g = blockIdx.x * GTC_WARPS + (threadIdx.x >> 5);
   if (g >= N * GT_T) return;
-  const int e = g / GT_T, t = g - e * GT_T, n = lane;
-  bool valid = false, vnow = false;
-  if (n < H) {
-    auto frame_pos = [&](int tt, float& x, float& y, float& m) {
-      if (tt == GT_T - 1) {
-        x = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
-        y = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
-        m = vis[(size_t)e * H + n] ? 1.0f : 0.0f;
-      } else {
-        const int slot = (newest + 1 + tt) % GT_T;
-        const size_t o = ((size_t)slot * N + e) * H + n;
-        x = ring_pos[2 * o]; y = ring_pos[2 * o + 1]; m = (float)ring_mask[o];
+  const int e = g / GT_T, t = g - e * GT_T;
+  int gc = 0, ec = 0;
+  for (int n0 = 0; n0 < H; n0 += 32) {
+    const int n = n0 + lane;
+    bool valid = false, vnow = false;
+    if (n < H) {
+      auto frame_pos = [&](int tt, float& x, float& y, float& m) {
+        if (tt == GT_T - 1) {
+          x = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
+          y = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
+          m = vis[(size_t)e * H + n] ? 1.0f : 0.0f;
+        } else {
+          const int slot = (newest + 1 + tt) % GT_T;
+          const size_t o = ((size_t)slot * N + e) * H + n;
+          x = ring_pos[2 * o]; y = ring_pos[2 * o + 1]; m = (float)ring_mask[o];
+        }
+      };
+      float x, y, m, xp = 0, yp = 0, mp = 0, xl_, yl_, ml_;
+      frame_pos(t, x, y, m);
+      frame_pos(GT_T - 1, xl_, yl_, ml_);
+      if (t > 0) frame_pos(t - 1, xp, yp, mp);
+      const float mrel = t == 0 ? m : mp * ml_;                  // interface.forward:77-78 (sic)
+      const float dx = t == 0 ? 0.0f : x - xp, dy = t == 0 ? 0.0f : y - yp;
+      const size_t r = (size_t)g * H + n;
+      rowm[r] = mrel;
+      inp[2 * r] = GT_INVALID * (1.0f - mrel) + dx * mrel;
+      inp[2 * r + 1] = GT_INVALID * (1.0f - mrel) + dy * mrel;
+      valid = mrel != 0.0f;
+      if (t == GT_T - 1) {
+        const size_t rd = (size_t)e * H + n;
+        fp[rd] = mrel; pos_last[2 * rd] = x; pos_last[2 * rd + 1] = y;
+        vnow = valid;
       }
-    };
-    float x, y, m, xp = 0, yp = 0, mp = 0, xl_, yl_, ml_;
-    frame_pos(t, x, y, m);
-    frame_pos(GT_T - 1, xl_, yl_, ml_);
-    if (t > 0) frame_pos(t - 1, xp, yp, mp);
-    const float mrel = t == 0 ? m : mp * ml_;                  // interface.forward:77-78 (sic)
-    const float dx = t == 0 ? 0.0f : x - xp, dy = t == 0 ? 0.0f : y - yp;
-    const size_t r = (size_t)g * H + n;
-    rowm[r] = mrel;
-    inp[2 * r] = GT_INVALID * (1.0f - mrel) + dx * mrel;
-    inp[2 * r + 1] = GT_INVALID * (1.0f - mrel) + dy * mrel;
-    valid = mrel != 0.0f;
+    }
+    gc += __popc(__ballot_sync(0xffffffffu, valid));
     if (t == GT_T - 1) {
-      const size_t rd = (size_t)e * H + n;
-      fp[rd] = mrel; pos_last[2 * rd] = x; pos_last[2 * rd + 1] = y;
-      vnow = valid;
+      ec += __popc(__ballot_sync(0xffffffffu, vnow));
+      // traj_buffer.append / mask_buffer.append.  Other groups of this launch read the newest frame from the observation,
+      // never from this slot (frame_pos), so the write cannot race with them.
+      if (n < H) {
+        const size_t o = ((size_t)newest * N + e) * H + n;
+        ring_pos[2 * o] = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
+        ring_pos[2 * o + 1] = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
+        ring_mask[o] = vis[(size_t)e * H + n] ? 1 : 0;
+      }
     }
   }
-  const uint32_t b = __ballot_sync(0xffffffffu, valid);
-  if (lane == 0) gcount[g] = __popc(b);
-  if (t == GT_T - 1) {
-    const uint32_t bn = __ballot_sync(0xffffffffu, vnow);
-    if (lane == 0) ecount[e] = __popc(bn);
-    // traj_buffer.append / mask_buffer.append.  Other groups of this launch read the newest frame from the observation,
-    // never from this slot (frame_pos), so the write cannot race with them.
-    if (n < H) {
-      const size_t o = ((size_t)newest * N + e) * H + n;
-      ring_pos[2 * o] = robot[e * 7] + sp2[((size_t)e * H + n) * 2];
-      ring_pos[2 * o + 1] = robot[e * 7 + 1] + sp2[((size_t)e * H + n) * 2 + 1];
-      ring_mask[o] = vis[(size_t)e * H + n] ? 1 : 0;
-    }
+  if (lane == 0) {
+    gcount[g] = gc;
+    if (t == GT_T - 1) ecount[e] = ec;
   }
 }
 
@@ -204,7 +221,8 @@ __global__ void __launch_bounds__(1024) gtc_scan_kernel(const int* __restrict__ 
   }
 }
 
-// compaction maps: cidx[r] (compact row or -1), crow[c] (source row), drow[d] (env * H + human of decode row d)
+// compaction maps: cidx[r] (compact row or -1), crow[c] (source row), drow[d] (env * H + human of decode row d).  One
+// warp per (env, frame) group, humans in chunks of 32 with a running offset: compact rows stay in ascending row order.
 __global__ void __launch_bounds__(GTC_WARPS * 32) gtc_index_kernel(int N, int H, const float* __restrict__ rowm, const float* __restrict__ fp,
                                                                     const int* __restrict__ gstart, const int* __restrict__ estart,
                                                                     int* __restrict__ cidx, int* __restrict__ crow, int* __restrict__ drow) {
@@ -213,17 +231,24 @@ __global__ void __launch_bounds__(GTC_WARPS * 32) gtc_index_kernel(int N, int H,
   const int g = blockIdx.x * GTC_WARPS + (threadIdx.x >> 5);
   if (g >= N * GT_T) return;
   const int e = g / GT_T, t = g - e * GT_T;
-  const size_t r = (size_t)g * H + lane;
-  const bool valid = lane < H && rowm[r] != 0.0f;
-  const uint32_t b = __ballot_sync(0xffffffffu, valid);
-  const int c = gstart[g] + __popc(b & ((1u << lane) - 1u));
-  if (lane < H) cidx[r] = valid ? c : -1;
-  if (valid) crow[c] = (int)r;
-  if (t == GT_T - 1) {
-    const size_t rd = (size_t)e * H + lane;
-    const bool vnow = lane < H && fp[rd] != 0.0f;
-    const uint32_t bn = __ballot_sync(0xffffffffu, vnow);
-    if (vnow) drow[estart[e] + __popc(bn & ((1u << lane) - 1u))] = (int)rd;
+  const uint32_t below = (1u << lane) - 1u;
+  int c0 = cn_ld_after_wait(gstart + g), d0 = t == GT_T - 1 ? cn_ld_after_wait(estart + e) : 0;
+  for (int n0 = 0; n0 < H; n0 += 32) {
+    const int n = n0 + lane;
+    const size_t r = (size_t)g * H + n;
+    const bool valid = n < H && rowm[r] != 0.0f;
+    const uint32_t b = __ballot_sync(0xffffffffu, valid);
+    const int c = c0 + __popc(b & below);
+    if (n < H) cidx[r] = valid ? c : -1;
+    if (valid) crow[c] = (int)r;
+    c0 += __popc(b);
+    if (t == GT_T - 1) {
+      const size_t rd = (size_t)e * H + n;
+      const bool vnow = n < H && fp[rd] != 0.0f;
+      const uint32_t bn = __ballot_sync(0xffffffffu, vnow);
+      if (vnow) drow[d0 + __popc(bn & below)] = (int)rd;
+      d0 += __popc(bn);
+    }
   }
 }
 
@@ -248,12 +273,13 @@ __global__ void __launch_bounds__(256) gtc_embed_kernel(GstTcW w, const int* __r
 }
 
 // attention within a group's compact rows [start[g], start[g+1]); the H - n masked neighbours enter the soft-max
-// denominator through their common key b_k (see the header of this section).  One CTA per group.
+// denominator through their common key b_k (see the header of this section).  One CTA of 8 * H threads per group, one
+// thread per (row, head); H * 192 floats of dynamic shared memory.
 __global__ void __launch_bounds__(8 * GT_MAXH) gtc_attn_kernel(int H, const int* __restrict__ start, const float* __restrict__ qkv,
                                                                const float* __restrict__ bk /* b_in + 64 */, __half* __restrict__ ah,
                                                                __half* __restrict__ al) {
   cn_pdl_prologue();
-  __shared__ __align__(16) float sq[GT_MAXH * 192];
+  extern __shared__ __align__(16) float sq[];
   const int c0 = cn_ld_after_wait(start + blockIdx.x), ng = cn_ld_after_wait(start + blockIdx.x + 1) - c0;
   if (ng <= 0) return;
   for (int i = threadIdx.x; i < ng * 48; i += blockDim.x)
@@ -429,21 +455,15 @@ int cn_gst_create(int num_envs, int human_num, int predict_steps, double robot_r
                   double collision_penalty, int device, cn_gst** out) {
   if (!out) return cn_set_error("cn_gst_create: null argument");
   *out = nullptr;
-  if (num_envs <= 0 || human_num <= 0 || human_num % 4 || predict_steps < 1 || predict_steps > GT_T)
-    return cn_set_error("cn_gst_create: need num_envs > 0, human_num %% 4 == 0 and 1 <= predict_steps <= %d (got %d, %d, %d)",
-                        GT_T, num_envs, human_num, predict_steps);
+  if (num_envs <= 0 || human_num <= 0 || human_num > GT_MAXH || predict_steps < 1 || predict_steps > GT_T)
+    return cn_set_error("cn_gst_create: need num_envs > 0, 1 <= human_num <= %d and 1 <= predict_steps <= %d (got %d, %d, %d)",
+                        GT_MAXH, GT_T, num_envs, human_num, predict_steps);
   int ndev = 0;
   cudaError_t err = cudaGetDeviceCount(&ndev);
   if (err != cudaSuccess || ndev == 0)
     return cn_set_error("cn_gst_create: no CUDA device (%s); this engine has no CPU fallback",
                         err == cudaSuccess ? "device count 0" : cudaGetErrorString(err));
   if (device < 0 || device >= ndev) return cn_set_error("cn_gst_create: bad device %d", device);
-  // human_num <= 24 is the range the predictor has always accepted: its first implementation ran one CTA per environment
-  // with the five observed frames in shared memory, which holds at most 24 humans.  The kernels of this file would hold
-  // GT_MAXH = 32; a wider range needs tests of its own.
-  if (human_num > 24)
-    return cn_set_error("cn_gst_create: human_num %d > 24 is not supported (the predictor's accepted range, set by the "
-                        "shared memory of its first, one-CTA-per-environment implementation)", human_num);
   cudaSetDevice(device);
   cn_gst* g = new cn_gst();
   g->N = num_envs; g->H = human_num; g->P = predict_steps; g->device = device;
@@ -452,6 +472,12 @@ int cn_gst_create(int num_envs, int human_num, int predict_steps, double robot_r
   CnLaunchCtx* ctx = &g->ctx;
   cn_launch_init(ctx, device);
   int rc = tc_set_attrs();
+  if (!rc && cudaFuncSetAttribute(gtc_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GT_MAXH * 192 * (int)sizeof(float)) !=
+                 cudaSuccess)
+    rc = cn_set_error("cn_gst_create: shared memory attribute of the attention kernel failed");
+  // workspace, sized for every row although only the live ones are used: 4125 bytes per observation row (R = N * 5 * H:
+  // fp32 X0 | QKV | O | X1 | GX, the split fp16 A operands, ring, masks, inputs, maps) + ~1.9 KB per decode row (N * H),
+  // 9.2 GB at N = 4096, H = 100
   const size_t R = (size_t)num_envs * GT_T * human_num, Rd = (size_t)num_envs * human_num;
   float* q = nullptr;
   if (!rc) rc = palloc(ctx, &g->ring_pos, R * 2);
@@ -570,7 +596,8 @@ int cn_gst_step(cn_gst* g, const float* d_robot_node, const float* d_spatial2, c
   const dim3 rows_grid((unsigned)(p->num_sms * 4)), grp_grid((unsigned)((G + GTC_WARPS - 1) / GTC_WARPS));
   auto encoder = [&](int maxrows, const int* cnt, int groups, const int* start) {
     gemm_tc(p, st, g->tX, g->tWin, maxrows, 192, 64, 64, g->w.bin, CN_ACT_NONE, out32(g->QKV, 192), cnt);
-    launch_k(p, gtc_attn_kernel, dim3((unsigned)groups), dim3((unsigned)(8 * H)), 0, st, H, start, g->QKV, g->w.bin + 64, g->tA.hi, g->tA.lo);
+    launch_k(p, gtc_attn_kernel, dim3((unsigned)groups), dim3((unsigned)(8 * H)), (size_t)H * 192 * sizeof(float), st, H, start,
+             g->QKV, g->w.bin + 64, g->tA.hi, g->tA.lo);
     gemm_tc(p, st, g->tA, g->tWout, maxrows, 64, 64, 64, g->w.bout, CN_ACT_NONE, out32(g->O, 64), cnt);
     launch_k(p, gtc_res_ln_kernel, rows_grid, dim3(256), 0, st, g->w, cnt, g->X0, g->O, g->X1, g->tY.hi, g->tY.lo);
     gemm_tc(p, st, g->tY, g->tW1, maxrows, 128, 64, 64, g->w.b1, CN_ACT_RELU, out16(g->tF), cnt);
@@ -603,8 +630,8 @@ int cn_gst_step(cn_gst* g, const float* d_robot_node, const float* d_spatial2, c
     }
     launch_k(p, gtc_h2p_kernel, rows_grid, dim3(256), 0, st, g->w, tt, cntD, g->drow, g->h32, g->pos_last, g->xin, g->mu_cum, g->pred);
   }
-  launch_k(p, gt_final_kernel, dim3((unsigned)N), dim3(32), 0, st, N, H, g->P, g->thr, g->collision_penalty, d_robot_node, d_spatial2,
-           g->fp, g->pred, d_reward, d_penalty, d_spatial_out);
+  launch_k(p, gt_final_kernel, dim3((unsigned)N), dim3((unsigned)((H + 31) / 32 * 32)), 0, st, N, H, g->P, g->thr,
+           g->collision_penalty, d_robot_node, d_spatial2, g->fp, g->pred, d_reward, d_penalty, d_spatial_out);
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return cn_set_error("cn_gst_step: %s", cudaGetErrorString(err));
   if (p->launch_error) { p->launch_error = false; return 1; }

@@ -116,7 +116,10 @@ int cn_fetch_sync(void *h_dst, const void *d_src, size_t bytes, int device, void
 
 /* BASELINE config 3: GST trajectory predictor + VecPretextNormalize processing (one chain of launches per step).
  * replaces: VecPretextNormalize.reset / process_obs_rew (rl/vec_env/vec_pretext_normalize.py:85-191) and
- * CrowdNavPredInterfaceMultiEnv.forward (gst_updated/scripts/wrapper/crowd_nav_interface_parallel.py:45-114).     */
+ * CrowdNavPredInterfaceMultiEnv.forward (gst_updated/scripts/wrapper/crowd_nav_interface_parallel.py:45-114).
+ * human_num = the wrapper's max_human_num (sim.human_num + sim.human_num_range): 1 to 128, as cn_env_create and
+ * cn_policy_create; anything else is refused.  Workspace ~4.1 KB per (environment, frame, human) row, N * 5 * H rows,
+ * plus ~1.9 KB per (environment, human): 9.2 GB at N = 4096, H = 100.                                          */
 typedef struct cn_gst cn_gst;
 int cn_gst_create(int num_envs, int human_num, int predict_steps, double robot_radius, double human_radius,
                   double collision_penalty, int device, cn_gst **out);

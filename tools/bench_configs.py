@@ -21,6 +21,9 @@ CONFIGS = {
     "c1_varnum": (dict(human_num=5, const_vel=0), 4096),
     # BASELINE config 3: CrowdSimPredRealGST-v0 + VecPretextNormalize (GST predictor), H = 20, N = 4096
     "c3": (dict(human_num=20), 4096),
+    # config 3 at config 4's and config 5's crowds (c3_h100: circle and arena x2, as c5)
+    "c3_h50": (dict(human_num=50), 4096),
+    "c3_h100": (dict(human_num=100, circle_radius=2 * 6 * 2 ** 0.5, arena_size=12.0), 4096),
 }
 
 
@@ -31,8 +34,8 @@ def run(name, steps, warmup):
     from crowdnav_prediction_attngraph_b200.storage import RolloutStorage
     kw, N = CONFIGS[name]
     dev = torch.device("cuda", 0)
-    if name == "c3":
-        return run_c3(kw, N, dev, steps, warmup)
+    if name.startswith("c3"):
+        return run_c3(name, kw, N, dev, steps, warmup)
     env = CudaCrowdVecEnv(num_envs=N, nenv_total=N, rank_offset=0, seed=425, device=dev, **kw)
 
     class Args(object):
@@ -101,12 +104,13 @@ def run(name, steps, warmup):
     del eng, policy, env
 
 
-def run_c3(kw, N, dev, steps, warmup):
+def run_c3(name, kw, N, dev, steps, warmup):
     import numpy as np
     import torch
     from crowdnav_prediction_attngraph_b200.vec_env import CudaPretextVecEnv
     from crowdnav_prediction_attngraph_b200.policy import Policy
     params = dict(np.load(os.path.join(REPO, "tests", "golden", "gst_params.npz")))
+    free0 = torch.cuda.mem_get_info(dev)[0]        # the engine's workspaces are cudaMalloc'd outside torch's allocator
     env = CudaPretextVecEnv(params, num_envs=N, nenv_total=N, rank_offset=0, seed=425, device=dev, **kw)
 
     class Args(object):
@@ -140,9 +144,12 @@ def run_c3(kw, N, dev, steps, warmup):
         env._process(raw, None)
     f1.record()
     torch.cuda.synchronize()
-    print(json.dumps({"config": "c3", "env_kwargs": kw, "envs": N, "ms_per_step": ms, "env_steps_per_s": N / ms * 1e3,
+    print(json.dumps({"config": name, "env_kwargs": kw, "envs": N, "ms_per_step": ms, "env_steps_per_s": N / ms * 1e3,
                       "gst_pretext_kernel_ms": f0.elapsed_time(f1) / 20,
-                      "valid_human_rows": int(eng.lib.cn_policy_last_rows(eng._h))}))
+                      "valid_human_rows": int(eng.lib.cn_policy_last_rows(eng._h)),
+                      "device_mem_gb": (free0 - torch.cuda.mem_get_info(dev)[0]) / 2 ** 30}))
+    env.close()
+    del eng, policy, env
 
 
 if __name__ == "__main__":

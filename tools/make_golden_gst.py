@@ -9,6 +9,12 @@ wrapper, recorded from the UNMODIFIED reference code (runs only in the build con
   tests/golden/gst_rollout.npz  CrowdSimPredRealGST-v0 environments stepped like the vec-env workers, their raw
                                 observations, and what VecPretextNormalize.process_obs_rew makes of them
 
+Opt-in modes (named on the command line; the default list is params, io, rollout) record larger crowds:
+  io_h13, io_h128               gst_io_h13.npz / gst_io_h128.npz: the predictor on 13 and 128 humans
+  rollout_h10_range3            gst_rollout_h10_range3.npz: 10 humans, human_num_range 3 (13 rows, humans join / leave)
+  rollout_h50                   gst_rollout_h50.npz: 50 humans
+  rollout_h100_x2               gst_rollout_h100_x2.npz: 100 humans, circle and arena x2 (BASELINE config 5's crowd)
+
 The reference objects are created without running their __init__ (which torch.load()s / unpickles files);
 the model arguments are the literal content of checkpoint/args.pickle.
 """
@@ -66,9 +72,8 @@ def make_params():
     print("wrote gst_params.npz", sum(v.numel() for v in sd.values()), "parameters")
 
 
-def make_io():
-    rng = np.random.RandomState(3)
-    N, H = 6, 20
+def make_io(name="gst_io.npz", N=6, H=20, seed=3):
+    rng = np.random.RandomState(seed)
     itf = build_interface(N)
     # smooth random walks + random visibility patterns (full, partial, never visible, appearing, disappearing)
     start = rng.uniform(-6, 6, (N, H, 1, 2))
@@ -83,12 +88,14 @@ def make_io():
     traj = np.where(mask, traj, -999.0)
     with torch.no_grad():
         out_traj, out_mask = itf.forward(torch.tensor(traj, dtype=torch.float32), torch.tensor(mask, dtype=torch.float32))
-    np.savez_compressed(os.path.join(GOLD, "gst_io.npz"), in_traj=traj.astype(np.float32), in_mask=mask,
+    np.savez_compressed(os.path.join(GOLD, name), in_traj=traj.astype(np.float32), in_mask=mask,
                         out_traj=out_traj.numpy(), out_mask=out_mask.numpy())
-    print("wrote gst_io.npz", out_traj.shape, float(out_mask.mean()))
+    print("wrote", name, out_traj.shape, float(out_mask.mean()))
 
 
-def make_rollout():
+def make_rollout(name="gst_rollout.npz", N=3, T=90, H=20, human_num_range=0, seed=425, scale=1):
+    """scale: factor on sim.circle_radius and sim.arena_size (2 for the 100-human crowd, which the reference's spawner
+    cannot place on the default circle)"""
     sys.argv = ["x", "--no-cuda", "--env-name", "CrowdSimPredRealGST-v0"]
     import gym
     import crowd_sim  # noqa: F401
@@ -96,9 +103,14 @@ def make_rollout():
     rvo2.ONLY_AGENT0 = False
     from crowd_nav.configs.config import Config
     from rl.vec_env.vec_pretext_normalize import VecPretextNormalize
-    N, T, H, seed = 3, 90, 20, 425
     cfg = Config()
     cfg.sim.human_num = H
+    # Config's sections are shared class objects: set every field a mode changes, so that modes run in one process
+    # do not see each other's settings (the values at scale 1 are the reference's defaults)
+    cfg.sim.human_num_range = human_num_range
+    cfg.sim.circle_radius = 6 * np.sqrt(2) * scale
+    cfg.sim.arena_size = 6 * scale
+    HM = H + human_num_range                      # VecPretextNormalize.max_human_num: rows of every observation
     cfg.sim.predict_method = "inferred"
     cfg.env.use_wrapper = True
     cfg.orca.neighbor_dist = 10
@@ -115,15 +127,15 @@ def make_rollout():
     w.config = cfg
     w.device = torch.device("cpu")
     w.num_envs = N
-    w.max_human_num = H
+    w.max_human_num = HM
     w.predictor = build_interface(N)
     w.pred_interval = int(cfg.data.pred_timestep // cfg.env.time_step)
     w.buffer_len = (GST_ARGS["obs_seq_len"] - 1) * w.pred_interval + 1
     # VecPretextNormalize.reset() without the venv call
-    w.traj_buffer = deque(list(-torch.ones((w.buffer_len, N, H, 2)) * 999), maxlen=w.buffer_len)
-    w.mask_buffer = deque(list(torch.zeros((w.buffer_len, N, H, 1), dtype=torch.bool)), maxlen=w.buffer_len)
+    w.traj_buffer = deque(list(-torch.ones((w.buffer_len, N, HM, 2)) * 999), maxlen=w.buffer_len)
+    w.mask_buffer = deque(list(torch.zeros((w.buffer_len, N, HM, 1), dtype=torch.bool)), maxlen=w.buffer_len)
     w.step_counter = 0
-    w.last_pos = torch.zeros(N, H, 2)
+    w.last_pos = torch.zeros(N, HM, 2)
 
     def stack(obs_list):
         out = {}
@@ -170,17 +182,36 @@ def make_rollout():
     for key in raw[0]:
         out["raw_" + key] = np.stack([r[key] for r in raw])
         out["fin_" + key] = np.stack([r[key] for r in fin])
-    out["meta"] = np.array([repr(dict(nenv=N, steps=T, human_num=H, seed=seed))])
-    np.savez_compressed(os.path.join(GOLD, "gst_rollout.npz"), **out)
-    print("wrote gst_rollout.npz; episodes:", rec["done"].sum(0), "penalised steps:",
+    meta = dict(nenv=N, steps=T, human_num=H, seed=seed)
+    if name != "gst_rollout.npz":                    # the default file's meta stays as it was recorded
+        meta.update(human_num_range=human_num_range, circle_radius=float(cfg.sim.circle_radius),
+                    arena_size=float(cfg.sim.arena_size))
+    out["meta"] = np.array([repr(meta)])
+    np.savez_compressed(os.path.join(GOLD, name), **out)
+    print("wrote %s; episodes:" % name, rec["done"].sum(0), "penalised steps:",
           int((np.abs(rec["reward"] - rec["reward_env"]) > 0).sum()))
 
 
+# opt-in crowds beyond the shipped 20 humans: mode -> (function, keyword arguments)
+EXTRA = {
+    "io_h13": (make_io, dict(name="gst_io_h13.npz", N=6, H=13, seed=13)),
+    "io_h128": (make_io, dict(name="gst_io_h128.npz", N=3, H=128, seed=128)),
+    "rollout_h10_range3": (make_rollout, dict(name="gst_rollout_h10_range3.npz", N=3, T=90, H=10, human_num_range=3)),
+    "rollout_h50": (make_rollout, dict(name="gst_rollout_h50.npz", N=2, T=60, H=50)),
+    "rollout_h100_x2": (make_rollout, dict(name="gst_rollout_h100_x2.npz", N=2, T=40, H=100, scale=2)),
+}
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["params", "io", "rollout"]
+    unknown = [m for m in which if m not in ("params", "io", "rollout") and m not in EXTRA]
+    if unknown:
+        sys.exit("unknown mode(s) %s; modes: params io rollout %s" % (unknown, " ".join(EXTRA)))
     if "params" in which:
         make_params()
     if "io" in which:
         make_io()
     if "rollout" in which:
         make_rollout()
+    for m in which:
+        if m in EXTRA:
+            EXTRA[m][0](**EXTRA[m][1])
