@@ -438,7 +438,31 @@ struct cn_gst {
   TcStoreMap GX_R, GX_Rd, GH_Rd;                             // store maps of the BN = 256 gate GEMMs' outputs, per row extent
   float* inp;                                                // [R, 2] masked input displacement of every (env, frame, human) row
   int *cidx, *crow, *gcount, *gstart, *ecount, *estart, *drow, *counts;   // compaction maps (see gtc_* kernels)
+  std::string stop_after;   // cn_internal_gst_stop_after: the next cn_gst_step returns after this stage (empty: never)
 };
+
+namespace {
+
+// Stages of one cn_gst_step in launch order, as cn_internal_gst_stop_after names them.  An encoder pass ("obs." over the
+// observation rows, "decK." in decoding step K = 1..4) is embed, qkv, attn, out, res_ln, ffn1, ffn2, res, gx; "lstmT"
+// is the LSTM cell of observed frame T (after its recurrent GEMM for T > 0); a decoding step K >= 1 continues with gh,
+// cell, h2p; "final" is the penalty / sort / write-out.
+std::vector<std::string> gst_stage_names() {
+  static const char* enc[] = {"embed", "qkv", "attn", "out", "res_ln", "ffn1", "ffn2", "res", "gx"};
+  std::vector<std::string> s = {"prep", "scan", "index"};
+  for (const char* e : enc) s.push_back(std::string("obs.") + e);
+  for (int t = 0; t < GT_T; ++t) s.push_back("lstm" + std::to_string(t));
+  s.push_back("dec0.h2p");
+  for (int k = 1; k < GT_T; ++k) {
+    const std::string p = "dec" + std::to_string(k) + ".";
+    for (const char* e : enc) s.push_back(p + e);
+    for (const char* e : {"gh", "cell", "h2p"}) s.push_back(p + e);
+  }
+  s.push_back("final");
+  return s;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -594,50 +618,140 @@ int cn_gst_step(cn_gst* g, const float* d_robot_node, const float* d_spatial2, c
   const int* cntR = g->counts;          // valid observation rows
   const int* cntD = g->counts + 1;      // humans visible in the newest frame
   const dim3 rows_grid((unsigned)(p->num_sms * 4)), grp_grid((unsigned)((G + GTC_WARPS - 1) / GTC_WARPS));
-  auto encoder = [&](int maxrows, const int* cnt, int groups, const int* start) {
+  // test hook (cn_internal_gst_stop_after): one string compare per stage while a stop is set, one empty() otherwise
+  const std::string stop = g->stop_after;
+  g->stop_after.clear();
+  auto at = [&](const std::string& pfx, const char* s) { return !stop.empty() && stop == pfx + s; };
+  auto finish = [&]() -> int {
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) return cn_set_error("cn_gst_step: %s", cudaGetErrorString(err));
+    if (p->launch_error) { p->launch_error = false; return 1; }
+    return 0;
+  };
+  // one encoder pass; true when the step stops inside it
+  auto encoder = [&](const std::string& pfx, int maxrows, const int* cnt, int groups, const int* start) {
     gemm_tc(p, st, g->tX, g->tWin, maxrows, 192, 64, 64, g->w.bin, CN_ACT_NONE, out32(g->QKV, 192), cnt);
+    if (at(pfx, "qkv")) return true;
     launch_k(p, gtc_attn_kernel, dim3((unsigned)groups), dim3((unsigned)(8 * H)), (size_t)H * 192 * sizeof(float), st, H, start,
              g->QKV, g->w.bin + 64, g->tA.hi, g->tA.lo);
+    if (at(pfx, "attn")) return true;
     gemm_tc(p, st, g->tA, g->tWout, maxrows, 64, 64, 64, g->w.bout, CN_ACT_NONE, out32(g->O, 64), cnt);
+    if (at(pfx, "out")) return true;
     launch_k(p, gtc_res_ln_kernel, rows_grid, dim3(256), 0, st, g->w, cnt, g->X0, g->O, g->X1, g->tY.hi, g->tY.lo);
+    if (at(pfx, "res_ln")) return true;
     gemm_tc(p, st, g->tY, g->tW1, maxrows, 128, 64, 64, g->w.b1, CN_ACT_RELU, out16(g->tF), cnt);
+    if (at(pfx, "ffn1")) return true;
     gemm_tc(p, st, g->tF, g->tW2, maxrows, 64, 128, 64, g->w.b2, CN_ACT_NONE, out32(g->O, 64), cnt);
+    if (at(pfx, "ffn2")) return true;
     launch_k(p, gtc_res_kernel, rows_grid, dim3(256), 0, st, cnt, g->X1, g->O, g->tXS.hi, g->tXS.lo);
+    if (at(pfx, "res")) return true;
     gemm_tc(p, st, g->tXS, g->tWih, maxrows, 256, 64, 256, g->w.bih, CN_ACT_NONE,
             out32(g->GX, 256, maxrows == R ? &g->GX_R : &g->GX_Rd), cnt);
+    return at(pfx, "gx");
   };
   launch_k(p, gtc_prep_kernel, grp_grid, dim3(GTC_WARPS * 32), 0, st, N, H, g->ring_pos, g->ring_mask, g->newest, d_robot_node, d_spatial2,
            d_visible, g->rowm, g->inp, g->gcount, g->ecount, g->fp, g->pos_last);
+  if (at("", "prep")) return finish();
   launch_k(p, gtc_scan_kernel, dim3(1), dim3(1024), 0, st, g->gcount, G, g->gstart, g->ecount, N, g->estart, g->counts);
+  if (at("", "scan")) return finish();
   launch_k(p, gtc_index_kernel, grp_grid, dim3(GTC_WARPS * 32), 0, st, N, H, g->rowm, g->fp, g->gstart, g->estart, g->cidx, g->crow,
            g->drow);
+  if (at("", "index")) return finish();
   launch_k(p, gtc_embed_kernel, rows_grid, dim3(256), 0, st, g->w, cntR, g->crow, g->inp, g->X0, g->tX.hi, g->tX.lo);
-  encoder(R, cntR, G, g->gstart);
+  if (at("obs.", "embed") || encoder("obs.", R, cntR, G, g->gstart)) return finish();
   // LSTM over the 5 observed frames, humans visible now only (h0 = c0 = 0: frame 0 has no recurrent GEMM, its
   // hidden-state gate term is b_hh)
   for (int t = 0; t < GT_T; ++t) {
     if (t > 0) gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
     launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, t, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
              g->c32, g->tHd.hi, g->tHd.lo);
+    if (!stop.empty() && stop == "lstm" + std::to_string(t)) return finish();
   }
   for (int tt = 0; tt < GT_T; ++tt) {
+    const std::string pfx = stop.empty() ? std::string() : "dec" + std::to_string(tt) + ".";
     if (tt > 0) {
       launch_k(p, gtc_embed_kernel, rows_grid, dim3(256), 0, st, g->w, cntD, (const int*)nullptr, g->xin, g->X0, g->tX.hi, g->tX.lo);
-      encoder(Rd, cntD, N, g->estart);
+      if (at(pfx, "embed") || encoder(pfx, Rd, cntD, N, g->estart)) return finish();
       gemm_tc(p, st, g->tHd, g->tWhh, Rd, 256, 64, 256, g->w.bhh, CN_ACT_NONE, out32(g->GH, 256, &g->GH_Rd), cntD);
+      if (at(pfx, "gh")) return finish();
       launch_k(p, gtc_cell_kernel, rows_grid, dim3(256), 0, st, H, -1, cntD, g->drow, g->cidx, g->GX, g->w.bih, g->w.bhh, g->GH, g->h32,
                g->c32, g->tHd.hi, g->tHd.lo);
+      if (at(pfx, "cell")) return finish();
     }
     launch_k(p, gtc_h2p_kernel, rows_grid, dim3(256), 0, st, g->w, tt, cntD, g->drow, g->h32, g->pos_last, g->xin, g->mu_cum, g->pred);
+    if (at(pfx, "h2p")) return finish();
   }
   launch_k(p, gt_final_kernel, dim3((unsigned)N), dim3((unsigned)((H + 31) / 32 * 32)), 0, st, N, H, g->P, g->thr,
            g->collision_penalty, d_robot_node, d_spatial2, g->fp, g->pred, d_reward, d_penalty, d_spatial_out);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return cn_set_error("cn_gst_step: %s", cudaGetErrorString(err));
-  if (p->launch_error) { p->launch_error = false; return 1; }
-  return 0;
+  return finish();
 }
 
 int64_t cn_gst_launch_count(cn_gst* g) { return g ? g->ctx.launches : 0; }
+
+// ---- test-only hooks (not in crowdnav_b200.h): tests/test_gpu_gst_stages.py reads the workspace stage by stage ----
+// Workspace buffer `name`: device pointer, rows, columns, row pitch (elements) and kind -- 0: fp32, 1: split fp16
+// (hi, lo) pair at *ptr / *ptr_lo (value = hi + lo), 2: int32, 3: uint8.  Row r starts at element r * *ld.  R = N*5*H
+// observation rows (compact: the first counts[0] are live), Rd = N*H decode rows (compact: the first counts[1]).
+//   ring_pos [5*N*H, 2], ring_mask [5*N*H] (slot-major [5][N][H]);  rowm [R], inp [R, 2], gcount [N*5], gstart [N*5+1],
+//   ecount [N], estart [N+1], counts [4], cidx / crow [R], drow [Rd], fp [Rd], pos_last [Rd, 2];
+//   X0 [R, 64], tX / tA / tY / tXS pairs [R, 64], QKV [R, 192], O / X1 [R, 64], tF pair [R, 128], GX [R, 256];
+//   GH [Rd, 256], h32 / c32 [Rd, 64], tHd pair [Rd, 64], xin / mu_cum [Rd, 2], pred [Rd, 10] (5 frames x (x, y)).
+// The decoding encoder reuses the observation encoder's buffers; see cn_internal_gst_stop_after.
+int cn_internal_gst_buffer(cn_gst* g, const char* name, void** ptr, void** ptr_lo, int* rows, int* cols, int* ld, int* kind) {
+  if (!g || !name || !ptr || !ptr_lo || !rows || !cols || !ld || !kind) return cn_set_error("cn_internal_gst_buffer: null argument");
+  const int R = g->N * GT_T * g->H, Rd = g->N * g->H, G = g->N * GT_T;
+  const std::string s(name);
+  *ptr_lo = nullptr;
+  auto set = [&](const void* q, int r, int c, int l, int k) { *ptr = (void*)q; *rows = r; *cols = c; *ld = l; *kind = k; return 0; };
+  auto f32 = [&](const float* q, int r, int c) { return set(q, r, c, c, 0); };
+  auto i32 = [&](const int* q, int r) { return set(q, r, 1, 1, 2); };
+  auto f16 = [&](const TcMat& t, int r, int c) { *ptr_lo = t.lo; return set(t.hi, r, c, t.pitch, 1); };
+  if (s == "ring_pos") return f32(g->ring_pos, R, 2);
+  if (s == "ring_mask") return set(g->ring_mask, R, 1, 1, 3);
+  if (s == "rowm") return f32(g->rowm, R, 1);
+  if (s == "inp") return f32(g->inp, R, 2);
+  if (s == "gcount") return i32(g->gcount, G);
+  if (s == "gstart") return i32(g->gstart, G + 1);
+  if (s == "ecount") return i32(g->ecount, g->N);
+  if (s == "estart") return i32(g->estart, g->N + 1);
+  if (s == "counts") return i32(g->counts, 4);
+  if (s == "cidx") return i32(g->cidx, R);
+  if (s == "crow") return i32(g->crow, R);
+  if (s == "drow") return i32(g->drow, Rd);
+  if (s == "fp") return f32(g->fp, Rd, 1);
+  if (s == "pos_last") return f32(g->pos_last, Rd, 2);
+  if (s == "X0") return f32(g->X0, R, 64);
+  if (s == "tX") return f16(g->tX, R, 64);
+  if (s == "QKV") return f32(g->QKV, R, 192);
+  if (s == "tA") return f16(g->tA, R, 64);
+  if (s == "O") return f32(g->O, R, 64);
+  if (s == "X1") return f32(g->X1, R, 64);
+  if (s == "tY") return f16(g->tY, R, 64);
+  if (s == "tF") return f16(g->tF, R, 128);
+  if (s == "tXS") return f16(g->tXS, R, 64);
+  if (s == "GX") return f32(g->GX, R, 256);
+  if (s == "GH") return f32(g->GH, Rd, 256);
+  if (s == "h32") return f32(g->h32, Rd, 64);
+  if (s == "c32") return f32(g->c32, Rd, 64);
+  if (s == "tHd") return f16(g->tHd, Rd, 64);
+  if (s == "xin") return f32(g->xin, Rd, 2);
+  if (s == "mu_cum") return f32(g->mu_cum, Rd, 2);
+  if (s == "pred") return f32(g->pred, Rd, GT_T * 2);
+  return cn_set_error("cn_internal_gst_buffer: unknown buffer '%s'", name);
+}
+
+// The next cn_gst_step returns right after stage `stage` (names: gst_stage_names), leaving the workspace as that stage
+// wrote it; null or "" clears.  The stopped step has still advanced the ring.  Off by default.
+int cn_internal_gst_stop_after(cn_gst* g, const char* stage) {
+  if (!g) return cn_set_error("cn_internal_gst_stop_after: null argument");
+  const std::string s(stage ? stage : "");
+  if (!s.empty()) {
+    bool known = false;
+    for (const std::string& n : gst_stage_names()) known = known || n == s;
+    if (!known) return cn_set_error("cn_internal_gst_stop_after: unknown stage '%s'", stage);
+  }
+  g->stop_after = s;
+  return 0;
+}
 
 }  // extern "C"
