@@ -7,6 +7,10 @@
 //   MultiheadAttention.out_proj  o  spatial_linear -> one 512 -> 256 projection (ReLU after)
 //   spatial_edge_layer folded into the robot side of the dot-product attention (u = W_s^T te)
 //
+// no_self_attn = 1 (the reference's use_self_attn = False, selfAttn_srnn_temp_node.py:340-345, :402-416): no
+// human-human attention; spatial_linear = Linear(W, 128), ReLU, Linear(128, 256), ReLU runs straight on the compacted
+// spatial_edges rows (layer 1 in the embed1 slot, layer 2 into sout) and feeds the unchanged robot-human attention.
+//
 // gemm_mode 0: every layer on the fp32 CUDA-core GEMM (cn_gemm_f32_kernel).
 // gemm_mode 1: every layer with K >= 64 on the wgmma 3xFP16 GEMM (cn_gemm_tc_kernel): activations
 //              travel between layers as (hi, lo) fp16 pairs written by the producing kernel's epilogue.
@@ -28,6 +32,9 @@
 struct cn_policy {
   cn_policy_config cfg;
   int N, H, Win, M;
+  bool nsa;           // cfg.no_self_attn: spatial_linear(spatial_edges), no human-human attention
+  const char* const* stage_names;   // this network's stages (kStageNames or kStageNamesNsa)
+  int num_stages;
   CnLaunchCtx lc;     // launch counter, PDL, first launch error, device allocations
   bool fuse_qkv;      // QKV projection + human-human attention in ONE kernel (cn_qkv_attn.cuh; opt-in, CN_FUSE_QKV=1)
   TcMat tWqkvH;       // folded QKV weight, rows head-major: [8][Q 64 | K 64 | V 64][512]
@@ -44,6 +51,7 @@ struct cn_policy {
   std::map<std::string, std::vector<float>> host;
   size_t ws_allocs;   // lc.allocs[0..ws_allocs) = workspace (kept); the rest = parameters of the last finalize
   // device parameters (fp32 kernel layouts)
+  // no_self_attn: W1 / b1 = spatial_linear.0 and W2 / b2 = spatial_linear.2; Wqkv ... bos are not allocated
   float *W1, *b1, *W2, *b2, *Wqkv, *bqkv, *Wos, *bos;
   float *Wr, *br, *Wet, *bet, *WsT, *bs, *Wa, *ba, *Wih, *bih, *Whh, *bhh, *Wo, *bo;
   float *Woac, *boac;      // (actor.0 | critic.0) o output_linear folded: 128 -> 512
@@ -105,9 +113,13 @@ void gemm(cn_policy* p, cudaStream_t st, const float* A, int lda, const float* W
 const char* kStageNames[] = {"pack_inputs", "embed1_gemm", "embed2_gemm", "qkv_gemm", "hh_attention",
                              "outproj_spatial_gemm", "robot_branch_join", "hr_attention", "gru", "actor_critic_heads"};
 const int kNumStages = sizeof(kStageNames) / sizeof(kStageNames[0]);
+// no_self_attn: the two spatial_linear layers, then the same tail as stages 6-9 above
+const char* kStageNamesNsa[] = {"pack_inputs", "spatial_linear0", "spatial_linear2", "robot_branch_join",
+                                "hr_attention", "gru", "actor_critic_heads"};
+const int kNumStagesNsa = sizeof(kStageNamesNsa) / sizeof(kStageNamesNsa[0]);
 
 inline void mark(cn_policy* p, cudaStream_t st, int i) {
-  p->lc.cur_stage = i < kNumStages ? kStageNames[i] : "end";
+  p->lc.cur_stage = i < p->num_stages ? p->stage_names[i] : "end";
   if (p->profile) cudaEventRecord(p->ev[i], st);
 }
 
@@ -127,13 +139,16 @@ int cn_policy_profile(cn_policy* p, int enable) {
 }
 int cn_policy_stage_count(void) { return kNumStages; }
 const char* cn_policy_stage_name(int i) { return (i >= 0 && i < kNumStages) ? kStageNames[i] : ""; }
+const char* cn_policy_handle_stage_name(cn_policy* p, int i) {
+  return (p && i >= 0 && i < p->num_stages) ? p->stage_names[i] : "";
+}
 int cn_policy_stage_ms(cn_policy* p, float* out, int n) {
   if (!p || !out) return cn_set_error("cn_policy_stage_ms: null argument");
   if (p->ev.empty()) return cn_set_error("cn_policy_stage_ms: profiling was never enabled");
   cudaSetDevice(p->cfg.device);
-  cudaError_t err = cudaEventSynchronize(p->ev[kNumStages]);
+  cudaError_t err = cudaEventSynchronize(p->ev[p->num_stages]);
   if (err != cudaSuccess) return cn_set_error("cn_policy_stage_ms: %s", cudaGetErrorString(err));
-  for (int i = 0; i < n && i < kNumStages; ++i) cudaEventElapsedTime(&out[i], p->ev[i], p->ev[i + 1]);
+  for (int i = 0; i < n && i < p->num_stages; ++i) cudaEventElapsedTime(&out[i], p->ev[i], p->ev[i + 1]);
   return 0;
 }
 
@@ -153,6 +168,9 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
   cn_policy* p = new cn_policy();
   p->cfg = *cfg;
   p->N = cfg->num_envs; p->H = cfg->human_num; p->Win = cfg->input_size; p->M = p->N * p->H;
+  p->nsa = cfg->no_self_attn != 0;
+  p->stage_names = p->nsa ? kStageNamesNsa : kStageNames;
+  p->num_stages = p->nsa ? kNumStagesNsa : kNumStages;
   p->finalized = false; p->profile = false;
   cn_launch_init(&p->lc, cfg->device);
   {
@@ -165,7 +183,7 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     const char* fq = getenv("CN_FUSE_QKV");
     // opt-in (CN_FUSE_QKV=1): parity green, but its attention is bound by the SM's shared-memory bandwidth, which it
     // shares with the operand fetch of the MMAs, and it does not overlap the next tile's MMAs (DESIGN.md 3.4b)
-    p->fuse_qkv = cfg->gemm_mode == 1 && p->qkv_chunks == 1 && (fq && fq[0] == '1') && p->N <= QA_MAX_ENVS && p->H <= 128;
+    p->fuse_qkv = !p->nsa && cfg->gemm_mode == 1 && p->qkv_chunks == 1 && (fq && fq[0] == '1') && p->N <= QA_MAX_ENVS && p->H <= 128;
   }
   cudaEventCreateWithFlags(&p->ev_tiles, cudaEventDisableTiming);
   cudaStreamCreateWithFlags(&p->st2, cudaStreamNonBlocking);
@@ -191,7 +209,8 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     if (!rc) rc = palloc(&p->lc, &q, 2 * N + 4);
     p->tile_tab = reinterpret_cast<int*>(q);
   }
-  WS(x16, M * 16); WS(e1, M * 128); WS(e2, M * 512); WS(qkv, M * 1536); WS(ao, M * 512); WS(sout, M * 256);
+  WS(x16, M * 16); WS(e1, M * 128); WS(sout, M * 256);
+  if (!p->nsa) { WS(e2, M * 512); WS(qkv, M * 1536); WS(ao, M * 512); }   // human-human attention only
   WS(xr, N * 16); WS(rs, N * 256); WS(t1, N * 128); WS(u, N * 256); WS(wv, N * 256); WS(h0, N * 128);
   WS(gi, N * 384); WS(gh, N * 384); WS(outb, N * 256); WS(ac1, N * 512); WS(a2, N * 256); WS(c2, N * 256);
 #undef WS
@@ -199,8 +218,8 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     // A operands: box rows = 128 (TC_BM)
     // per-human rows feed the BN = 256 instance, per-environment rows the BN = 64 one
     rc = tc_alloc(&p->lc, p->tE1, Mi, 128, TC_BM, tc_box_k(256));
-    if (!rc) rc = tc_alloc(&p->lc, p->tE2, Mi, 512, TC_BM, tc_box_k(256));
-    if (!rc) rc = tc_alloc(&p->lc, p->tAo, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc && !p->nsa) rc = tc_alloc(&p->lc, p->tE2, Mi, 512, TC_BM, tc_box_k(256));
+    if (!rc && !p->nsa) rc = tc_alloc(&p->lc, p->tAo, Mi, 512, TC_BM, tc_box_k(256));
     if (!rc) rc = tc_alloc(&p->lc, p->tRs, Ni, 256, TC_BM, tc_box_k(64));
     if (!rc) rc = tc_alloc(&p->lc, p->tT1, Ni, 128, TC_BM, tc_box_k(64));   // [enc | te] then [enc | emb]
     if (!rc) rc = tc_view(p->tTe, p->tT1, 64, Ni, 64, TC_BM);           // te = columns 64..127
@@ -212,10 +231,10 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     if (!rc) rc = tc_view(p->tA1, p->tAc1, 0, Ni, 256, TC_BM);          // actor.0 half
     if (!rc) rc = tc_view(p->tC1, p->tAc1, 256, Ni, 256, TC_BM);        // critic.0 half
     // fp32 outputs of the BN = 256 GEMMs (qkv, outproj_spatial)
-    if (!rc) rc = make_store_map(&p->qkv_st, p->qkv, 4, Mi, 1536, 1536);
+    if (!rc && !p->nsa) rc = make_store_map(&p->qkv_st, p->qkv, 4, Mi, 1536, 1536);
     if (!rc) rc = make_store_map(&p->sout_st, p->sout, 4, Mi, 256, 256);
     if (!rc) rc = tc_set_attrs();
-    if (!rc) {
+    if (!rc && !p->nsa) {
       err = cudaFuncSetAttribute(cn_qkv_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, QA_SMEM_BYTES);
       if (err != cudaSuccess) rc = cn_set_error("cudaFuncSetAttribute(qkv_attn): %s", cudaGetErrorString(err));
     }
@@ -252,23 +271,37 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
   cudaSetDevice(p->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
   const int Win = p->Win;
+  // the per-human chain: embedding_layer -> q/k/v_linear -> multihead_attn -> spatial_linear (512 -> 256), or with
+  // no_self_attn spatial_linear alone (W -> 128 -> 256) and no spatial_attn.* key at all
+  const std::vector<float> *w1, *b1, *w2, *b2, *wq = nullptr, *bq = nullptr, *wk = nullptr, *bk = nullptr;
+  const std::vector<float> *wvv = nullptr, *bvv = nullptr, *win = nullptr, *bin = nullptr, *wout = nullptr;
+  const std::vector<float> *bout = nullptr, *wsl = nullptr, *bsl = nullptr;
+#define GETP(var, key, count) if (!(var = get(p, key, (count)))) return 1
+  if (p->nsa) {
+    GETP(w1, "base.spatial_linear.0.weight", (size_t)128 * Win);
+    GETP(b1, "base.spatial_linear.0.bias", 128);
+    GETP(w2, "base.spatial_linear.2.weight", (size_t)256 * 128);
+    GETP(b2, "base.spatial_linear.2.bias", 256);
+  } else {
+    GETP(w1, "base.spatial_attn.embedding_layer.0.weight", (size_t)128 * Win);
+    GETP(b1, "base.spatial_attn.embedding_layer.0.bias", 128);
+    GETP(w2, "base.spatial_attn.embedding_layer.2.weight", (size_t)512 * 128);
+    GETP(b2, "base.spatial_attn.embedding_layer.2.bias", 512);
+    GETP(wq, "base.spatial_attn.q_linear.weight", (size_t)512 * 512);
+    GETP(bq, "base.spatial_attn.q_linear.bias", 512);
+    GETP(wk, "base.spatial_attn.k_linear.weight", (size_t)512 * 512);
+    GETP(bk, "base.spatial_attn.k_linear.bias", 512);
+    GETP(wvv, "base.spatial_attn.v_linear.weight", (size_t)512 * 512);
+    GETP(bvv, "base.spatial_attn.v_linear.bias", 512);
+    GETP(win, "base.spatial_attn.multihead_attn.in_proj_weight", (size_t)1536 * 512);
+    GETP(bin, "base.spatial_attn.multihead_attn.in_proj_bias", 1536);
+    GETP(wout, "base.spatial_attn.multihead_attn.out_proj.weight", (size_t)512 * 512);
+    GETP(bout, "base.spatial_attn.multihead_attn.out_proj.bias", 512);
+    GETP(wsl, "base.spatial_linear.0.weight", (size_t)256 * 512);
+    GETP(bsl, "base.spatial_linear.0.bias", 256);
+  }
+#undef GETP
 #define GET(var, key, count) const std::vector<float>* var = get(p, key, (count)); if (!var) return 1
-  GET(w1, "base.spatial_attn.embedding_layer.0.weight", (size_t)128 * Win);
-  GET(b1, "base.spatial_attn.embedding_layer.0.bias", 128);
-  GET(w2, "base.spatial_attn.embedding_layer.2.weight", (size_t)512 * 128);
-  GET(b2, "base.spatial_attn.embedding_layer.2.bias", 512);
-  GET(wq, "base.spatial_attn.q_linear.weight", (size_t)512 * 512);
-  GET(bq, "base.spatial_attn.q_linear.bias", 512);
-  GET(wk, "base.spatial_attn.k_linear.weight", (size_t)512 * 512);
-  GET(bk, "base.spatial_attn.k_linear.bias", 512);
-  GET(wvv, "base.spatial_attn.v_linear.weight", (size_t)512 * 512);
-  GET(bvv, "base.spatial_attn.v_linear.bias", 512);
-  GET(win, "base.spatial_attn.multihead_attn.in_proj_weight", (size_t)1536 * 512);
-  GET(bin, "base.spatial_attn.multihead_attn.in_proj_bias", 1536);
-  GET(wout, "base.spatial_attn.multihead_attn.out_proj.weight", (size_t)512 * 512);
-  GET(bout, "base.spatial_attn.multihead_attn.out_proj.bias", 512);
-  GET(wsl, "base.spatial_linear.0.weight", (size_t)256 * 512);
-  GET(bsl, "base.spatial_linear.0.bias", 256);
   GET(wr, "base.robot_linear.0.weight", (size_t)256 * 9);
   GET(br, "base.robot_linear.0.bias", 256);
   GET(wt, "base.attn.temporal_edge_layer.0.weight", (size_t)64 * 256);
@@ -327,48 +360,55 @@ int cn_policy_finalize(cn_policy* p, void* stream) {
   UP(Wa2, *wa2); UP(ba2, *ba2); UP(Wc2, *wc2); UP(bc2, *bc2);
   UP(wv_, *wcl); UP(bv, *bcl); UP(Wm, *wm); UP(bm, *bm); UP(logstd, *ls);
 #undef UP
-  // folded projections
-  float *d_win = nullptr, *d_bin = nullptr, *d_wl[3] = {nullptr, nullptr, nullptr}, *d_bl[3] = {nullptr, nullptr, nullptr};
-  float *d_wout = nullptr, *d_bout = nullptr, *d_wsl = nullptr, *d_bsl = nullptr;
-  if (!rc) rc = upload(p, &d_win, *win);
-  if (!rc) rc = upload(p, &d_bin, *bin);
-  const std::vector<float>* wl[3] = {wq, wk, wvv};
-  const std::vector<float>* bl[3] = {bq, bk, bvv};
-  for (int i = 0; i < 3 && !rc; ++i) { rc = upload(p, &d_wl[i], *wl[i]); if (!rc) rc = upload(p, &d_bl[i], *bl[i]); }
-  if (!rc) rc = upload(p, &d_wout, *wout);
-  if (!rc) rc = upload(p, &d_bout, *bout);
-  if (!rc) rc = upload(p, &d_wsl, *wsl);
-  if (!rc) rc = upload(p, &d_bsl, *bsl);
-  if (!rc) rc = palloc(&p->lc, &p->Wqkv, (size_t)1536 * 512);
-  if (!rc) rc = palloc(&p->lc, &p->bqkv, 1536);
-  if (!rc) rc = palloc(&p->lc, &p->Wos, (size_t)256 * 512);
-  if (!rc) rc = palloc(&p->lc, &p->bos, 256);
   if (!rc) rc = palloc(&p->lc, &p->Woac, (size_t)512 * 128);
   if (!rc) rc = palloc(&p->lc, &p->boac, 512);
   if (rc) return rc;
-  for (int i = 0; i < 3; ++i) {
-    // Wf_i = Win_i (512x512) @ Wl_i (512x512);  bf_i = Win_i @ bl_i + bin_i
-    cn_fold_mm_kernel<<<dim3(4, 512), 128, 0, st>>>(d_win + (size_t)i * 512 * 512, d_wl[i],
-                                                     p->Wqkv + (size_t)i * 512 * 512, 512, 512, 512);
-    cn_fold_mv_kernel<<<4, 128, 0, st>>>(d_win + (size_t)i * 512 * 512, d_bl[i], d_bin + i * 512, p->bqkv + i * 512, 512, 512);
-  }
-  // Wos = Wsl (256x512) @ Wout (512x512);  bos = Wsl @ bout + bsl
-  cn_fold_mm_kernel<<<dim3(4, 256), 128, 0, st>>>(d_wsl, d_wout, p->Wos, 256, 512, 512);
-  cn_fold_mv_kernel<<<2, 128, 0, st>>>(d_wsl, d_bout, d_bsl, p->bos, 256, 512);
   // Woac = [actor.0 ; critic.0] (512x256) @ output_linear (256x128);  boac = [actor.0 ; critic.0] @ bo + bac1
   // (output_linear has no activation and feeds only the two MLPs, selfAttn_srnn_temp_node.py:438-447)
   cn_fold_mm_kernel<<<dim3(1, 512), 128, 0, st>>>(p->Wac1, p->Wo, p->Woac, 512, 128, 256);
   cn_fold_mv_kernel<<<4, 128, 0, st>>>(p->Wac1, p->bo, p->bac1, p->boac, 512, 256);
+  if (!p->nsa) {
+    // folded projections of the human-human attention
+    float *d_win = nullptr, *d_bin = nullptr, *d_wl[3] = {nullptr, nullptr, nullptr}, *d_bl[3] = {nullptr, nullptr, nullptr};
+    float *d_wout = nullptr, *d_bout = nullptr, *d_wsl = nullptr, *d_bsl = nullptr;
+    if (!rc) rc = upload(p, &d_win, *win);
+    if (!rc) rc = upload(p, &d_bin, *bin);
+    const std::vector<float>* wl[3] = {wq, wk, wvv};
+    const std::vector<float>* bl[3] = {bq, bk, bvv};
+    for (int i = 0; i < 3 && !rc; ++i) { rc = upload(p, &d_wl[i], *wl[i]); if (!rc) rc = upload(p, &d_bl[i], *bl[i]); }
+    if (!rc) rc = upload(p, &d_wout, *wout);
+    if (!rc) rc = upload(p, &d_bout, *bout);
+    if (!rc) rc = upload(p, &d_wsl, *wsl);
+    if (!rc) rc = upload(p, &d_bsl, *bsl);
+    if (!rc) rc = palloc(&p->lc, &p->Wqkv, (size_t)1536 * 512);
+    if (!rc) rc = palloc(&p->lc, &p->bqkv, 1536);
+    if (!rc) rc = palloc(&p->lc, &p->Wos, (size_t)256 * 512);
+    if (!rc) rc = palloc(&p->lc, &p->bos, 256);
+    if (rc) return rc;
+    for (int i = 0; i < 3; ++i) {
+      // Wf_i = Win_i (512x512) @ Wl_i (512x512);  bf_i = Win_i @ bl_i + bin_i
+      cn_fold_mm_kernel<<<dim3(4, 512), 128, 0, st>>>(d_win + (size_t)i * 512 * 512, d_wl[i],
+                                                       p->Wqkv + (size_t)i * 512 * 512, 512, 512, 512);
+      cn_fold_mv_kernel<<<4, 128, 0, st>>>(d_win + (size_t)i * 512 * 512, d_bl[i], d_bin + i * 512, p->bqkv + i * 512, 512, 512);
+    }
+    // Wos = Wsl (256x512) @ Wout (512x512);  bos = Wsl @ bout + bsl
+    cn_fold_mm_kernel<<<dim3(4, 256), 128, 0, st>>>(d_wsl, d_wout, p->Wos, 256, 512, 512);
+    cn_fold_mv_kernel<<<2, 128, 0, st>>>(d_wsl, d_bout, d_bsl, p->bos, 256, 512);
+  }
   if (p->cfg.gemm_mode == 1) {
     // fp16 (hi, lo) split of the tensor-core weights, pre-scaled by 2^6 (exact) so lo stays normal.
     // B-tile rows: 256 for the per-human layers (large M), 64 for the per-environment layers.
+    // no_self_attn: W2 is spatial_linear.2 [256, 128]; there is no Wqkv / Wos (rows = 0: skipped)
+    const int nh = p->nsa ? 0 : 1;
     struct { float* src; TcMat* t; int rows, k, bn; } tw[13] = {
         {p->Woac, &p->tWoac, 512, 128, 64},
-        {p->W2, &p->tW2, 512, 128, 256},    {p->Wqkv, &p->tWqkv, 1536, 512, 256}, {p->Wos, &p->tWos, 256, 512, 256},
+        {p->W2, &p->tW2, p->nsa ? 256 : 512, 128, 256}, {p->Wqkv, &p->tWqkv, 1536 * nh, 512, 256},
+        {p->Wos, &p->tWos, 256 * nh, 512, 256},
         {p->Wet, &p->tWet, 128, 256, 64},   {p->WsT, &p->tWsT, 256, 64, 64},      {p->Wa, &p->tWa, 64, 256, 64},
         {p->Wih, &p->tWih, 384, 128, 64},   {p->Whh, &p->tWhh, 384, 128, 64},     {p->Wo, &p->tWo, 256, 128, 64},
         {p->Wac1, &p->tWac1, 512, 256, 64}, {p->Wa2, &p->tWa2, 256, 256, 64},     {p->Wc2, &p->tWc2, 256, 256, 64}};
     for (auto& t : tw) {
+      if (!t.rows) continue;
       rc = tc_alloc(&p->lc, *t.t, t.rows, t.k, t.bn, tc_box_k(t.bn));
       if (rc) return rc;
       split16(&p->lc, st, t.src, 64.0f, t.t->hi, t.t->lo, (size_t)t.rows * t.k);
@@ -444,59 +484,66 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
                                                      p->tE1.hi, p->tE1.lo);
   } else gemm(p, st, p->x16, 16, p->W1, 16, p->b1, p->e1, 128, M, 128, 16, CN_ACT_RELU, 0, ALL, mc);
   mark(p, st, 2);
-  if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 512, 128, 256, p->b2, CN_ACT_RELU, out16(p->tE2), mc);
-  else gemm(p, st, p->e1, 128, p->W2, 128, p->b2, p->e2, 512, M, 512, 128, CN_ACT_RELU, 0, ALL, mc);
-  mark(p, st, 3);
-  if (tcm) {
-    // Optional experiment (CN_QKV_CHUNKS=2): QKV projection + attention in two row chunks split at an environment
-    // boundary so that chunk 0's attention (side stream) overlaps chunk 1's GEMM.  Off by default: at H = 20 the
-    // attention is load-latency bound, not L2-capacity bound, and the overlap does not pay; at H = 50 and 100 it
-    // saves 0.4-3 % of the forward (DESIGN.md 3.4c).
-    const int* mid = p->row_start + N / 2;
-    __half* ah = p->tAo.hi;
-    __half* al = p->tAo.lo;
-    if (p->fuse_qkv) {
-      // one kernel: projection tile (128 rows of whole environments x one head's Q | K | V) -> attention -> tAo
-      cudaStreamWaitEvent(st, p->ev_tiles, 0);                 // tile table from the side stream
-      launch_k(&p->lc, cn_qkv_attn_kernel, dim3(p->lc.num_sms), dim3(QA_THREADS), QA_SMEM_BYTES, st, p->qa_ah, p->qa_al, p->qa_bh,
-               p->qa_bl, p->bqkvH, 1.0f / 64.0f, p->tile_tab, p->row_start, p->row_env, ah, al,
-               getenv("CN_QA_DBG") ? atoi(getenv("CN_QA_DBG")) : 0);
-      mark(p, st, 4);
-    } else if (p->qkv_chunks == 1) {
-      gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
-      mark(p, st, 4);
-      launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
-                                                                             nullptr, ah, al);
-    } else {
-    gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mid);
-    cudaEventRecord(p->ev_fork3, st);
-    cudaStreamWaitEvent(p->st3, p->ev_fork3, 0);
-    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 32 / p->attn_warps), dim3(p->attn_warps * 32), 0, p->st3, p->qkv, p->row_start, p->row_env, mid, nullptr,
-                                                                              nullptr, ah, al);
-    cudaEventRecord(p->ev_join3, p->st3);
-    gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
-    mark(p, st, 4);
-    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
-                                                                           ah, al);
-    cudaStreamWaitEvent(st, p->ev_join3, 0);
-    }
+  if (p->nsa) {
+    // no_self_attn: spatial_linear.2 + ReLU is the last per-human layer, straight into sout
+    if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 256, 128, 256, p->b2, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
+    else gemm(p, st, p->e1, 128, p->W2, 128, p->b2, p->sout, 256, M, 256, 128, CN_ACT_RELU, 0, ALL, mc);
   } else {
-    gemm(p, st, p->e2, 512, p->Wqkv, 512, p->bqkv, p->qkv, 1536, M, 1536, 512, CN_ACT_NONE, 0, ALL, mc);
-    mark(p, st, 4);
-    launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, p->mc, nullptr,
-                                                                           p->ao, nullptr, nullptr);
+    if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 512, 128, 256, p->b2, CN_ACT_RELU, out16(p->tE2), mc);
+    else gemm(p, st, p->e1, 128, p->W2, 128, p->b2, p->e2, 512, M, 512, 128, CN_ACT_RELU, 0, ALL, mc);
+    mark(p, st, 3);
+    if (tcm) {
+      // Optional experiment (CN_QKV_CHUNKS=2): QKV projection + attention in two row chunks split at an environment
+      // boundary so that chunk 0's attention (side stream) overlaps chunk 1's GEMM.  Off by default: at H = 20 the
+      // attention is load-latency bound, not L2-capacity bound, and the overlap does not pay; at H = 50 and 100 it
+      // saves 0.4-3 % of the forward (DESIGN.md 3.4c).
+      const int* mid = p->row_start + N / 2;
+      __half* ah = p->tAo.hi;
+      __half* al = p->tAo.lo;
+      if (p->fuse_qkv) {
+        // one kernel: projection tile (128 rows of whole environments x one head's Q | K | V) -> attention -> tAo
+        cudaStreamWaitEvent(st, p->ev_tiles, 0);                 // tile table from the side stream
+        launch_k(&p->lc, cn_qkv_attn_kernel, dim3(p->lc.num_sms), dim3(QA_THREADS), QA_SMEM_BYTES, st, p->qa_ah, p->qa_al, p->qa_bh,
+                 p->qa_bl, p->bqkvH, 1.0f / 64.0f, p->tile_tab, p->row_start, p->row_env, ah, al,
+                 getenv("CN_QA_DBG") ? atoi(getenv("CN_QA_DBG")) : 0);
+        mark(p, st, 4);
+      } else if (p->qkv_chunks == 1) {
+        gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
+        mark(p, st, 4);
+        launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
+                                                                               nullptr, ah, al);
+      } else {
+      gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mid);
+      cudaEventRecord(p->ev_fork3, st);
+      cudaStreamWaitEvent(p->st3, p->ev_fork3, 0);
+      launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 32 / p->attn_warps), dim3(p->attn_warps * 32), 0, p->st3, p->qkv, p->row_start, p->row_env, mid, nullptr,
+                                                                                nullptr, ah, al);
+      cudaEventRecord(p->ev_join3, p->st3);
+      gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
+      mark(p, st, 4);
+      launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
+                                                                             ah, al);
+      cudaStreamWaitEvent(st, p->ev_join3, 0);
+      }
+    } else {
+      gemm(p, st, p->e2, 512, p->Wqkv, 512, p->bqkv, p->qkv, 1536, M, 1536, 512, CN_ACT_NONE, 0, ALL, mc);
+      mark(p, st, 4);
+      launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, p->mc, nullptr,
+                                                                             p->ao, nullptr, nullptr);
+    }
+    mark(p, st, 5);
+    if (tcm) gemm_tc(&p->lc, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
+    else gemm(p, st, p->ao, 512, p->Wos, 512, p->bos, p->sout, 256, M, 256, 512, CN_ACT_RELU, 0, ALL, mc);
   }
-  mark(p, st, 5);
-  if (tcm) gemm_tc(&p->lc, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
-  else gemm(p, st, p->ao, 512, p->Wos, 512, p->bos, p->sout, 256, M, 256, 512, CN_ACT_RELU, 0, ALL, mc);
-  // 2. join the robot branch
-  mark(p, st, 6);
+  // 2. join the robot branch (stage indices from here on: the last four of the handle's stages)
+  const int tail = p->num_stages - 4;
+  mark(p, st, tail);
   cudaStreamWaitEvent(st, p->ev_join, 0);
-  mark(p, st, 7);
+  mark(p, st, tail + 1);
   launch_k(&p->lc, cn_hr_attention_kernel<false>, dim3((N + 3) / 4), dim3(128), 0, st, p->sout, p->u, p->t1, 128, 64, p->bs, p->row_start, 0, 0,
                                                       N, H, p->wv, tcm ? p->tWv.hi : nullptr, tcm ? p->tWv.lo : nullptr, 256);
   // 3. GRU: emb overwrites the te half of t1 -> t1 = [enc | emb] = GRU input (gh came from the side stream)
-  mark(p, st, 8);
+  mark(p, st, tail + 2);
   if (tcm) {
     TcOut o; o.oh = p->tT1.hi + 64; o.ol = p->tT1.lo + 64; o.ldh = 128;
     gemm_tc(&p->lc, st, p->tWv, p->tWa, N, 64, 256, 64, p->ba, CN_ACT_RELU, o);
@@ -508,7 +555,7 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   launch_k(&p->lc, cn_gru_gate_kernel, dim3((N * 128 + 255) / 256), dim3(256), 0, st, p->gi, p->gh, p->h0, N, d->h_out, tcm ? p->tH1.hi : nullptr,
                                                             tcm ? p->tH1.lo : nullptr);
   // 4. output_linear, actor / critic MLPs (critic.2 on the side stream), heads
-  mark(p, st, 9);
+  mark(p, st, tail + 3);
   if (tcm) {
     gemm_tc(&p->lc, st, p->tH1, p->tWoac, N, 512, 128, 64, p->boac, CN_ACT_TANH, out16(p->tAc1));     // [actor.0 | critic.0]
     cudaEventRecord(p->ev_fork2, st);
@@ -527,7 +574,7 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   cudaStreamWaitEvent(st, p->ev_join2, 0);
   launch_k(&p->lc, cn_heads_kernel, dim3((N + 3) / 4), dim3(128), 0, st, p->a2, 256, p->c2, 256, p->wv_, p->bv, p->Wm, p->bm, p->logstd, d->noise, N,
                                                d->value, d->action, d->log_prob, d->action_mean);
-  mark(p, st, kNumStages);
+  mark(p, st, p->num_stages);
   cudaError_t err = cudaGetLastError();
   if (p->lc.launch_error) { p->lc.launch_error = false; return 1; }      // cn_last_error names the stage
   if (err != cudaSuccess) return cn_set_error("cn_policy_act launch: %s", cudaGetErrorString(err));
@@ -557,6 +604,8 @@ int64_t cn_policy_last_rows(cn_policy* p) {
 //   t1: the GRU input [enc | emb].  The edge embedding (stage gru) overwrites the te half of [enc | te]; in
 //       gemm_mode 1 only the split pair is overwritten and "t1.f32" keeps [enc | te].
 //   h1: gemm_mode 1 only (gemm_mode 0 reads the caller's h_out).
+// no_self_attn: "e1" is the output of spatial_linear.0 + ReLU and "sout" that of spatial_linear.2 + ReLU; e2, qkv, ao
+// and the folded Wqkv / bqkv / Wos / bos do not exist.
 int cn_internal_policy_buffer(cn_policy* p, const char* name, void** ptr, void** ptr_lo, int* rows, int* cols, int* ld,
                               int* kind) {
   if (!p || !name || !ptr || !ptr_lo || !rows || !cols || !ld || !kind)
@@ -573,6 +622,8 @@ int cn_internal_policy_buffer(cn_policy* p, const char* name, void** ptr, void**
   if (s == "row_start") return i32(p->row_start, N + 1);
   if (s == "row_env") return i32(p->row_env, M);
   if (s == "mc") return i32(p->mc, 1);
+  if (p->nsa && (s == "e2" || s == "qkv" || s == "ao" || s == "Wqkv" || s == "bqkv" || s == "Wos" || s == "bos"))
+    return cn_set_error("cn_internal_policy_buffer: '%s' does not exist without human-human attention (no_self_attn)", name);
   if (s == "e1") return tcm ? f16(p->tE1, M, 128) : f32(p->e1, M, 128, 128);
   if (s == "e2") return tcm ? f16(p->tE2, M, 512) : f32(p->e2, M, 512, 512);
   if (s == "qkv") {

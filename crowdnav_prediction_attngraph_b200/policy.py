@@ -36,9 +36,11 @@ def _ortho(m, gain=1.0):
 
 
 class _Params(nn.Module):
-    """Parameter container with the reference's module tree (names drive the state_dict keys)."""
+    """Parameter container with the reference's module tree (names drive the state_dict keys).  self_attn=False is the
+    reference's use_self_attn = False (selfAttn_srnn_temp_node.py:340-345): no spatial_attn, and spatial_linear =
+    Linear(input_size, 128), ReLU, Linear(128, 256), ReLU with the orthogonal sqrt(2) init."""
 
-    def __init__(self, input_size):
+    def __init__(self, input_size, self_attn=True):
         super().__init__()
         g = math.sqrt(2)
         base = nn.Module()
@@ -62,14 +64,18 @@ class _Params(nn.Module):
         base.critic_linear = _ortho(nn.Linear(256, 1), g)
         base.robot_linear = nn.Sequential(_ortho(nn.Linear(9, 256), g), nn.ReLU())
         base.human_node_final_linear = _ortho(nn.Linear(256, 2), g)   # unused by forward (reference :338)
-        sa = nn.Module()
-        sa.embedding_layer = nn.Sequential(nn.Linear(input_size, 128), nn.ReLU(), nn.Linear(128, 512), nn.ReLU())
-        sa.q_linear = nn.Linear(512, 512)
-        sa.v_linear = nn.Linear(512, 512)
-        sa.k_linear = nn.Linear(512, 512)
-        sa.multihead_attn = nn.MultiheadAttention(512, 8)
-        base.spatial_attn = sa
-        base.spatial_linear = nn.Sequential(_ortho(nn.Linear(512, 256), g), nn.ReLU())
+        if self_attn:
+            sa = nn.Module()
+            sa.embedding_layer = nn.Sequential(nn.Linear(input_size, 128), nn.ReLU(), nn.Linear(128, 512), nn.ReLU())
+            sa.q_linear = nn.Linear(512, 512)
+            sa.v_linear = nn.Linear(512, 512)
+            sa.k_linear = nn.Linear(512, 512)
+            sa.multihead_attn = nn.MultiheadAttention(512, 8)
+            base.spatial_attn = sa
+            base.spatial_linear = nn.Sequential(_ortho(nn.Linear(512, 256), g), nn.ReLU())
+        else:
+            base.spatial_linear = nn.Sequential(_ortho(nn.Linear(input_size, 128), g), nn.ReLU(),
+                                                _ortho(nn.Linear(128, 256), g), nn.ReLU())
         self.base = base
         dist = nn.Module()
         dist.fc_mean = _ortho(nn.Linear(256, 2))
@@ -77,22 +83,26 @@ class _Params(nn.Module):
         self.dist = dist
 
 
-def make_reference_like_state_dict(input_size=12, seed=0):
-    """Random-init parameters with the reference's initialisers (orthogonal where it uses them)."""
+def make_reference_like_state_dict(input_size=12, seed=0, self_attn=True):
+    """Random-init parameters with the reference's initialisers (orthogonal where it uses them); self_attn=False: the
+    use_self_attn = False network."""
     gen_state = torch.random.get_rng_state()
     torch.manual_seed(seed)
-    sd = {k: v.detach().clone() for k, v in _Params(input_size).state_dict().items()}
+    sd = {k: v.detach().clone() for k, v in _Params(input_size, self_attn).state_dict().items()}
     torch.random.set_rng_state(gen_state)
     return sd
 
 
 class CudaPolicy(object):
-    """Thin handle on cn_policy: upload a reference state_dict, run the rollout forward."""
+    """Thin handle on cn_policy: upload a reference state_dict, run the rollout forward.  self_attn=False runs the
+    reference's use_self_attn = False network (cn_policy_config.no_self_attn)."""
 
-    def __init__(self, num_envs, human_num, input_size=12, device="cuda:0", gemm_mode=1):
+    def __init__(self, num_envs, human_num, input_size=12, device="cuda:0", gemm_mode=1, self_attn=True):
         self._setup(num_envs, human_num, input_size, device)
+        self.self_attn = bool(self_attn)
         cfg = _capi.CnPolicyConfig(num_envs, human_num, input_size,
-                                   self.device.index if self.device.index is not None else 0, gemm_mode)
+                                   self.device.index if self.device.index is not None else 0, gemm_mode,
+                                   0 if self.self_attn else 1)
         self._h = C.c_void_p()
         _capi.check(self.lib, self.lib.cn_policy_create(C.byref(cfg), C.byref(self._h)), "cn_policy_create")
 
@@ -191,6 +201,18 @@ class CudaPolicy(object):
 
     def launch_count(self):
         return int(self.lib.cn_policy_launch_count(self._h))
+
+    def profile(self, enable=True):
+        _capi.check(self.lib, self.lib.cn_policy_profile(self._h, int(enable)), "cn_policy_profile")
+
+    def stage_ms(self):
+        """{stage: ms} of the last act, under this handle's own stage names (profiling must have been enabled with
+        profile(True) before it)."""
+        n = self.lib.cn_policy_stage_count()
+        out = (C.c_float * n)()
+        _capi.check(self.lib, self.lib.cn_policy_stage_ms(self._h, out, n), "cn_policy_stage_ms")
+        names = [self.lib.cn_policy_handle_stage_name(self._h, i).decode() for i in range(n)]
+        return {k: float(out[i]) for i, k in enumerate(names) if k}
 
     def close(self):
         if self._h:
@@ -347,8 +369,33 @@ def _hh_attention(q, k, v, valid):
     return torch.matmul(torch.softmax(s, dim=-1), v)
 
 
+# The widths every kernel has fixed, by the argument that sets them in the reference's arguments.py, and which base's
+# module reads it: selfAttn_merge_SRNN's EndRNN / EdgeAttention_M never read human_human_edge_embedding_size (its node
+# GRU is RNNBase(edge=False)); SRNN's edge RNNs do.
+WIDTHS = (("human_node_rnn_size", HIDDEN, ("selfAttn_merge_srnn", "srnn")),
+          ("human_human_edge_rnn_size", 256, ("selfAttn_merge_srnn", "srnn")),
+          ("human_node_output_size", 256, ("selfAttn_merge_srnn", "srnn")),
+          ("human_node_embedding_size", 64, ("selfAttn_merge_srnn", "srnn")),
+          ("human_human_edge_embedding_size", 64, ("srnn",)),
+          ("attention_size", 64, ("selfAttn_merge_srnn", "srnn")))
+
+
+def check_widths(args, base):
+    """Refuse an argument file whose network widths differ from the ones the kernels are built for."""
+    if args is None:
+        return
+    for name, width, bases in WIDTHS:
+        v = getattr(args, name, width)
+        if base in bases and int(v) != width:
+            raise NotImplementedError("%s = %r: the engine's %s network is built for %s = %d only"
+                                      % (name, v, base, name, width))
+
+
 class Policy(nn.Module):
-    """Drop-in for rl.networks.model.Policy(obs_space.spaces, action_space, base_kwargs=args, base=...)."""
+    """Drop-in for rl.networks.model.Policy(obs_space.spaces, action_space, base_kwargs=args, base=...).
+
+    args.use_self_attn = False (selfAttn_merge_srnn only; True when absent) is the reference's ablation without
+    human-human attention.  args.use_hr_attn is accepted and changes nothing: the reference never reads it."""
 
     def __init__(self, obs_shape, action_space, base=None, base_kwargs=None):
         super().__init__()
@@ -362,12 +409,15 @@ class Policy(nn.Module):
             env_type = getattr(args, 'env_type', 'crowd_sim') if args is not None else 'crowd_sim'
             if env_type != 'crowd_sim':
                 raise NotImplementedError("base='srnn' runs env_type 'crowd_sim' only (got %r)" % (env_type,))
+        check_widths(args, 'srnn' if self.dsrnn else 'selfAttn_merge_srnn')
+        # the reference's SRNN ignores use_self_attn (srnn_model.py); older argument files lack it (True)
+        self.self_attn = self.dsrnn or bool(getattr(args, 'use_self_attn', True))
         sp = obs_shape['spatial_edges'].shape
         self.human_num, self.input_size = int(sp[0]), int(sp[1])
         self.nenv = int(getattr(args, 'num_processes', 1)) if args is not None else 1
         self.seq_length = int(getattr(args, 'seq_length', 30)) if args is not None else 30
         self.nminibatch = int(getattr(args, 'num_mini_batch', 2)) if args is not None else 2
-        p = (_SrnnParams if self.dsrnn else _Params)(self.input_size)
+        p = _SrnnParams(self.input_size) if self.dsrnn else _Params(self.input_size, self.self_attn)
         self.base = p.base
         # attributes the reference's callers read / write on `actor_critic.base` (test.py:148, rl/evaluation.py:15-21)
         self.base.nenv = self.nenv
@@ -394,7 +444,7 @@ class Policy(nn.Module):
                 self._cuda = CudaDsrnn(N, self.human_num, self.input_size, device=device)
             else:
                 self._cuda = CudaPolicy(N, self.human_num, self.input_size, device=device,
-                                        gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")))
+                                        gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")), self_attn=self.self_attn)
             self._cuda_version = -1
         # parameter objects are fixed after construction: walk the module tree once, then only read the
         # version counters (the tree walk alone cost ~0.1 ms of host time per act)
@@ -446,11 +496,49 @@ class Policy(nn.Module):
         valid = torch.arange(H, device=sp.device)[None, :] < n[:, None]
         rs = b.robot_linear(torch.cat([inputs['temporal_edges'].reshape(T * N, 2),
                                        inputs['robot_node'].reshape(T * N, 7)], -1).to(dt))
+        B = T * N
+        use_tc = sp.is_cuda and dt == torch.float32 and getattr(self, "update_kernels", os.environ.get("CN_UPDATE_KERNELS", "1") == "1")
+        if use_tc:
+            from . import update_ops as uo
+
+        def pad(x):
+            out = x.new_zeros(B, H, x.shape[-1])
+            out[valid] = x
+            return out
+
+        def compact_layout():
+            row_start = torch.zeros(B + 1, dtype=torch.int32, device=sp.device)
+            row_start[1:] = torch.cumsum(n, 0)
+            return row_start, torch.repeat_interleave(torch.arange(B, device=sp.device, dtype=torch.int32), n)
+        if not self.self_attn:
+            # use_self_attn = False: spatial_linear straight on the spatial edges (selfAttn_srnn_temp_node.py:408-410)
+            sl = b.spatial_linear
+            hs_c = row_env = None
+            if not getattr(self, "pack_valid_rows", True):
+                hs = sl(sp)
+            elif use_tc:
+                e1 = torch.relu(F.linear(sp[valid], sl[0].weight, sl[0].bias))       # K = W <= 12: torch
+                hs_c = uo.linear_tc(e1, sl[2].weight, sl[2].bias, 1)                  # [Mc, 256], compact
+                hs = None
+                row_env = compact_layout()[1]
+            else:
+                hs = pad(sl(sp[valid]))
+        else:
+            hs, hs_c, row_env = self._hh_features(sp, n, valid, B, use_tc, pad, compact_layout)
+        return self._tail(rs, hs, hs_c, row_env, valid, h0, masks, T, N)
+
+    def _hh_features(self, sp, n, valid, B, use_tc, pad, compact_layout):
+        """Human-human attention then spatial_linear: hs [B, H, 256] (padded rows zero), or with the update kernels
+        (hs = None) the compact hs_c [Mc, 256] and its row_env."""
+        b = self.base
+        H = self.human_num
         sa = b.spatial_attn
         mha = sa.multihead_attn
         wq, wk, wv = mha.in_proj_weight.chunk(3, 0)
         bq, bk, bv = mha.in_proj_bias.chunk(3, 0)
-        B = T * N
+        if use_tc:
+            from . import update_ops as uo
+        hs_c = row_env = None
 
         def heads(x):
             return x.reshape(B, H, 8, 64).transpose(1, 2)
@@ -463,18 +551,11 @@ class Policy(nn.Module):
             sp_p = sp[valid]                                             # [Mc, W]
             # update kernels (SURVEY §8f row 3): the three 128/512-wide per-row layers forward + backward on the wgmma
             # 3xFP16 GEMM and the attention core over compacted rows; plain torch ops on CPU or with CN_UPDATE_KERNELS=0
-            use_tc = sp.is_cuda and dt == torch.float32 and getattr(self, "update_kernels", os.environ.get("CN_UPDATE_KERNELS", "1") == "1")
             if use_tc:
-                from . import update_ops as uo
                 e1 = torch.relu(F.linear(sp_p, sa.embedding_layer[0].weight, sa.embedding_layer[0].bias))   # K = 12: torch
                 e = uo.linear_tc(e1, sa.embedding_layer[2].weight, sa.embedding_layer[2].bias, 1)
             else:
                 e = sa.embedding_layer(sp_p)
-
-            def pad(x):
-                out = x.new_zeros(B, H, x.shape[-1])
-                out[valid] = x
-                return out
             # The same exact folds as the rollout engine, written so that autograd sees them: in_proj o q/k/v_linear
             # is ONE 512 -> 1536 projection whose weight is the (differentiable) product of the two parameter
             # matrices, and out_proj o spatial_linear one 512 -> 256 projection: the per-row GEMMs of forward AND
@@ -489,9 +570,7 @@ class Policy(nn.Module):
             b_os = sl.weight @ mha.out_proj.bias + sl.bias
             if use_tc:
                 qkv = uo.linear_tc(e, w_qkv, b_qkv, 0)
-                row_start = torch.zeros(B + 1, dtype=torch.int32, device=sp.device)
-                row_start[1:] = torch.cumsum(n, 0)
-                row_env = torch.repeat_interleave(torch.arange(B, device=sp.device, dtype=torch.int32), n)
+                row_start, row_env = compact_layout()
                 o = uo.hh_attention_rows(qkv, row_start, row_env)
                 hs_c = uo.linear_tc(o, w_os, b_os, 1)          # [Mc, 256]: stays compact through the robot-human attention
                 hs = None
@@ -509,8 +588,18 @@ class Policy(nn.Module):
             o = F.scaled_dot_product_attention(q, k, v, attn_mask=amask)
             o = mha.out_proj(o.transpose(1, 2).reshape(B, H, 512))
             hs = b.spatial_linear(o)
+        return hs, hs_c, row_env
+
+    def _tail(self, rs, hs, hs_c, row_env, valid, h0, masks, T, N):
+        """Robot-human attention, node GRU, actor / critic over the per-human features hs [B, H, 256], or the compact
+        hs_c [Mc, 256] with its row_env (update kernels)."""
+        b = self.base
+        H = self.human_num
+        B = T * N
         tc_rows = hs is None                       # update kernels: per-sample layers on the tensor cores as well
         if tc_rows:
+            from . import update_ops as uo
+
             def lin(x, layer, act=0):
                 return uo.linear_tc(x, layer.weight, layer.bias, act)
         else:

@@ -220,12 +220,18 @@ typedef struct cn_policy_config {
   int32_t input_size;   /* spatial_edges row width (12 for Pred envs, 2 for VarNum)            */
   int32_t device;
   int32_t gemm_mode;    /* 0: fp32 CUDA-core GEMM; 1: wgmma 3xFP16 error-compensated GEMM      */
+  int32_t no_self_attn; /* 0: the paper's network.  1: the reference's use_self_attn = False      */
+                        /* ablation: no human-human attention; the parameters are               */
+                        /* base.spatial_linear.0 [128, input_size] and .2 [256, 128] (+ biases)  */
+                        /* and no base.spatial_attn.* key; CN_FUSE_QKV / CN_ATTN_R /             */
+                        /* CN_QKV_CHUNKS have no effect.  A zeroed field keeps today's network.  */
 } cn_policy_config;
 
 int cn_policy_create(const cn_policy_config *cfg, cn_policy **out);
 int cn_policy_destroy(cn_policy *pol);
 
 /* Upload one state_dict tensor by its reference key (SURVEY.md §2.3), float32 host data.       */
+/* cn_policy_finalize names the first missing key of the configured network.                    */
 int cn_policy_set_param(cn_policy *pol, const char *key, const float *h_data, size_t count);
 /* Fold/convert the uploaded parameters into the kernels' layouts; call after all set_param.    */
 int cn_policy_finalize(cn_policy *pol, void *stream);
@@ -254,10 +260,14 @@ int64_t cn_policy_last_rows(cn_policy *pol);
 /* Per-stage device timing of cn_policy_act (CUDA events on the launching stream), for bench.py's
  * roofline line.  enable != 0 records events around every stage of subsequent calls;
  * cn_policy_stage_ms synchronises and writes the last call's stage durations (ms) into out[0..n).
- * Stage names: cn_policy_stage_name(i), i < cn_policy_stage_count().                            */
+ * Stage names: cn_policy_stage_name(i), i < cn_policy_stage_count().                            *
+ * A no_self_attn handle has fewer stages (spatial_linear0, spatial_linear2 in place of the five *
+ * human-human stages): cn_policy_handle_stage_name(pol, i) names the handle's own stage i and   *
+ * returns "" past its last one; cn_policy_stage_count() bounds every handle's count.            */
 int cn_policy_profile(cn_policy *pol, int enable);
 int cn_policy_stage_count(void);
 const char *cn_policy_stage_name(int i);
+const char *cn_policy_handle_stage_name(cn_policy *pol, int i);
 int cn_policy_stage_ms(cn_policy *pol, float *out, int n);
 
 /* ------------------------------------------------------------------------------------------ */

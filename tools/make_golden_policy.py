@@ -7,6 +7,15 @@ shipped checkpoint trained_models/GST_predictor_rand/checkpoints/41665.pt, so fi
 small (no 10 MB weight file in git); inputs are observations recorded in tests/golden/env_*.npz.
 A second fixture stores the outputs of the shipped checkpoint itself on the same inputs
 (only compared in this container, where the checkpoint exists).
+
+--no-self-attn writes only the fixtures of the reference's ablation without human-human attention
+(args.use_self_attn = False set on the argument namespace): policy_nsa_h20 (W = 12, env_pred_h20),
+policy_nsa_h50 (W = 12, env_pred_h50_rand) and policy_nsa_varnum (W = 2, CrowdSimVarNum-v0,
+env_varnum_h20_vis_rand).  Weights: tests/policy_no_self_attn_ref.synth_state_dict_nsa (the fill above for every key
+shared with the full network; spatial_linear.0 / .2 from the reference's orthogonal initialiser with seeded
+generators).  Each file also holds the reference module's state_dict keys and shapes.
+
+    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_policy.py [--no-self-attn]
 """
 import os
 import sys
@@ -32,12 +41,13 @@ def param_fill(state_dict, seed, scales):
     return out
 
 
-def build_reference_policy(env_name, H, W, nenv):
+def build_reference_policy(env_name, H, W, nenv, use_self_attn=True):
     sys.argv = ["x", "--no-cuda", "--env-name", env_name, "--num-processes", str(nenv)]
     import gym
     from arguments import get_args
     from rl.networks.model import Policy
     args = get_args()
+    args.use_self_attn = use_self_attn
     obs_space = {"robot_node": gym.spaces.Box(-np.inf, np.inf, (1, 7)),
                  "temporal_edges": gym.spaces.Box(-np.inf, np.inf, (1, 2)),
                  "spatial_edges": gym.spaces.Box(-np.inf, np.inf, (H, W)),
@@ -84,10 +94,41 @@ def main():
 
 
 
+def no_self_attn_fixtures():
+    sys.path.insert(0, os.path.join(REPO, "tests"))
+    from tests.policy_no_self_attn_ref import synth_state_dict_nsa
+    for name, env_name, env_file, H, W in [("policy_nsa_h20", "CrowdSimPred-v0", "env_pred_h20", 20, 12),
+                                           ("policy_nsa_h50", "CrowdSimPred-v0", "env_pred_h50_rand", 50, 12),
+                                           ("policy_nsa_varnum", "CrowdSimVarNum-v0", "env_varnum_h20_vis_rand", 20, 2)]:
+        g = long_h20_recording() if env_file == "env_pred_h20" else np.load(os.path.join(REPO, "tests", "golden", env_file + ".npz"))
+        T, N = g["actions"].shape[:2]
+        B = 64
+        idx = np.random.RandomState(0).choice((T + 1) * N, B, replace=False)
+        take = lambda k: torch.from_numpy(g["ob_" + k].reshape((T + 1) * N, *g["ob_" + k].shape[2:])[idx].astype(np.float32))
+        obs = {k: take(k) for k in ["robot_node", "temporal_edges", "spatial_edges", "detected_human_num"]}
+        gen = torch.Generator().manual_seed(123)
+        h = torch.randn(B, 1, 128, generator=gen) * 0.5
+        masks = (torch.rand(B, 1, generator=gen) > 0.1).float()
+        pol = build_reference_policy(env_name, H, W, B, use_self_attn=False)
+        sd = pol.state_dict()
+        pol.load_state_dict(synth_state_dict_nsa(sd))
+        rnn = {"human_node_rnn": h.clone(), "human_human_edge_rnn": torch.zeros(B, H + 1, 256)}
+        with torch.no_grad():
+            value, feat, hx = pol.base({k: v.clone() for k, v in obs.items()}, rnn, masks.clone(), infer=True)
+            mean = pol.dist.fc_mean(feat)
+        keys = sorted(sd.keys())
+        print(name, "value range", float(value.min()), float(value.max()), "mean abs max", float(mean.abs().max()),
+              "detected", float(obs["detected_human_num"].mean()))
+        np.savez_compressed(os.path.join(REPO, "tests", "golden", name + ".npz"),
+                            h=h.numpy(), masks=masks.numpy(), **{"ob_" + k: v.numpy() for k, v in obs.items()},
+                            synth_value=value.numpy(), synth_mean=mean.numpy(), synth_h=hx["human_node_rnn"].numpy(),
+                            sd_keys=np.array(keys), sd_shapes=np.array([str(tuple(sd[k].shape)) for k in keys]))
+
+
 def long_h20_recording():
     """The 260-step env_pred_h20 rollout of the reference (the committed fixture keeps only its first steps)."""
     import make_golden
     return make_golden.run_case("env_pred_h20", dict(make_golden.CASES["env_pred_h20"], steps=make_golden.LONG_H20_STEPS))
 
 if __name__ == "__main__":
-    main()
+    no_self_attn_fixtures() if "--no-self-attn" in sys.argv[1:] else main()

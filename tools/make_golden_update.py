@@ -13,7 +13,11 @@ parameter tensor, its sum / abs-sum / first 4 entries after the update.  A secon
 holds the update's change of up to 512 seeded entries of EVERY parameter tensor (the full 10 MB of weights do not
 fit a fixture), compared entry by entry by tests/test_update_parity_reference.py.
 
-    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_update.py
+--no-self-attn records the same two files for the reference's ablation without human-human attention
+(args.use_self_attn = False; weights tests/policy_no_self_attn_ref.synth_state_dict_nsa):
+update_nsa_t30_n8.npz and update_nsa_t30_n8_entries.npz.
+
+    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_update.py [--no-self-attn]
 """
 import os
 import sys
@@ -32,6 +36,15 @@ WINDOWS = None      # filled by pick_windows
 HYPER = dict(clip_param=0.2, ppo_epoch=2, num_mini_batch=2, value_loss_coef=0.5, entropy_coef=0.01,
              lr=4e-5, eps=1e-5, max_grad_norm=0.5)
 SEED_GEN = 777
+USE_SELF_ATTN = "--no-self-attn" not in sys.argv[1:]
+
+
+def synth(template):
+    if USE_SELF_ATTN:
+        from policy_fixture import synth_state_dict
+        return synth_state_dict(template)
+    from policy_no_self_attn_ref import synth_state_dict_nsa
+    return synth_state_dict_nsa(template)
 
 
 def pick_windows(done):
@@ -65,11 +78,12 @@ def cut_rollout(g):
 
 def reference_objects():
     from make_golden_policy import build_reference_policy
-    pol = build_reference_policy("CrowdSimPred-v0", H, W, N)
+    argv = sys.argv
+    pol = build_reference_policy("CrowdSimPred-v0", H, W, N, use_self_attn=USE_SELF_ATTN)
+    sys.argv = argv
     pol.base.nminibatch = HYPER["num_mini_batch"]
     pol.base.seq_length = T
-    from policy_fixture import synth_state_dict
-    pol.load_state_dict(synth_state_dict(pol.state_dict()))
+    pol.load_state_dict(synth(pol.state_dict()))
     return pol
 
 
@@ -153,9 +167,8 @@ ENTRIES_PER_TENSOR = 512
 def sample_entries(pol):
     """Seeded sample of the update's parameter change: up to ENTRIES_PER_TENSOR flat indices of every tensor (sorted
     keys), the entries' change from the synthetic initial weights."""
-    from policy_fixture import synth_state_dict
     sd = pol.state_dict()
-    pre = synth_state_dict(sd)
+    pre = synth(sd)
     rng = np.random.default_rng(2024)
     keys, idx, off, delta = sorted(sd.keys()), [], [0], []
     for k in keys:
@@ -170,8 +183,9 @@ def sample_entries(pol):
 
 if __name__ == "__main__":
     out, ref_pol = run_reference()
-    p = os.path.join(REPO, "tests", "golden", "update_t30_n8.npz")
+    tag = "update_t30_n8" if USE_SELF_ATTN else "update_nsa_t30_n8"
+    p = os.path.join(REPO, "tests", "golden", tag + ".npz")
     np.savez_compressed(p, **out)
-    np.savez_compressed(os.path.join(REPO, "tests", "golden", "update_t30_n8_entries.npz"), **sample_entries(ref_pol))
+    np.savez_compressed(os.path.join(REPO, "tests", "golden", tag + "_entries.npz"), **sample_entries(ref_pol))
     print("wrote", p, os.path.getsize(p), "bytes; losses", out["losses"], "entropy", out["mb_entropy"],
           "dones per env", out["done"].sum(0))

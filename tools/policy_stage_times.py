@@ -6,7 +6,11 @@ of detected humans (mean about 4.2), takes the stage times from cn_policy_profil
 median over the timed calls.  It also prints, computed from the shapes, the rows, output tiles, L2 -> shared-memory
 operand bytes and issued FLOPs of the three BN = 256 GEMMs (embed2, qkv, outproj), with the card name and power limit.
 
-    python tools/policy_stage_times.py [--envs 4096] [--humans 20] [--reps 300] [--warmup 30] [--seed 0]
+--no-self-attn times the network without human-human attention (the reference's use_self_attn = False) instead: its
+stages, the whole act (CUDA events around cn_policy_act alone, profiling off) and the device-resident rollout rate of
+CrowdSimPred-v0 (env step + act into the rollout storage, as bench.py's value rate, at --humans).
+
+    python tools/policy_stage_times.py [--envs 4096] [--humans 20] [--reps 300] [--warmup 30] [--seed 0] [--no-self-attn]
 """
 import argparse
 import ctypes as C
@@ -27,6 +31,7 @@ BM = 128            # output tile rows of cn_gemm_tc_kernel
 BN = 256            # output tile columns of the per-human GEMMs
 # (name, stage, K, N) of the per-human 3xFP16 GEMMs
 GEMMS = [("embed2", "embed2_gemm", 128, 512), ("qkv", "qkv_gemm", 512, 1536), ("outproj", "outproj_spatial_gemm", 512, 256)]
+GEMMS_NSA = [("spatial2", "spatial_linear2", 128, 256)]      # no_self_attn: its only per-human tensor-core GEMM
 
 
 def gemm_counts(rows, K, N):
@@ -59,6 +64,8 @@ def main():
     ap.add_argument("--reps", type=int, default=300)
     ap.add_argument("--warmup", type=int, default=30)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--no-self-attn", action="store_true", help="the network without human-human attention")
+    ap.add_argument("--rollout-steps", type=int, default=300, help="timed steps of the rollout rate (--no-self-attn)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("policy_stage_times.py needs a CUDA device")
@@ -76,11 +83,14 @@ def main():
     masks = torch.ones(N, 1, device=dev)
     noise = torch.randn(N, 2, generator=g).to(dev)
 
-    pol = CudaPolicy(N, H, Win, device=dev)
-    pol.load_state_dict(make_reference_like_state_dict(input_size=Win, seed=0))
+    self_attn = not a.no_self_attn
+    pol = CudaPolicy(N, H, Win, device=dev, self_attn=self_attn)
+    pol.load_state_dict(make_reference_like_state_dict(input_size=Win, seed=0, self_attn=self_attn))
     lib = pol.lib
     ns = lib.cn_policy_stage_count()
-    names = [lib.cn_policy_stage_name(i).decode() for i in range(ns)]
+    names = [lib.cn_policy_handle_stage_name(pol._h, i).decode() for i in range(ns)]
+    names = [k for k in names if k]
+    ns = len(names)
     lib.cn_policy_profile(pol._h, 1)
     buf = (C.c_float * ns)()
     samples = {k: [] for k in names}
@@ -109,15 +119,74 @@ def main():
     print("%-8s %6s %6s %6s %12s %10s %8s %12s %12s" % ("gemm", "K", "N", "tiles", "L2->smem MB", "issued GF", "alg GF",
                                                         "issued TF/s", "L2->smem TB/s"))
     shapes = {}
-    for name, stage, K, Ncol in GEMMS:
+    for name, stage, K, Ncol in (GEMMS if self_attn else GEMMS_NSA):
         c = gemm_counts(rows, K, Ncol)
         shapes[name] = dict(K=K, N=Ncol, tiles=c["tiles"], l2_smem_MB=round(c["l2_smem_MB"], 1),
                             issued_GFLOP=round(c["issued_GFLOP"], 2), alg_GFLOP=round(c["alg_GFLOP"], 2))
         print("%-8s %6d %6d %6d %12.1f %10.2f %8.2f %12.1f %12.2f" % (
             name, K, Ncol, c["tiles"], c["l2_smem_MB"], c["issued_GFLOP"], c["alg_GFLOP"], c["issued_GFLOP"] / med[stage],
             c["l2_smem_MB"] / 1e3 / med[stage]))
-    print(json.dumps(dict(card=info, N=N, H=H, rows=rows, reps=a.reps, median_ms={k: round(v, 5) for k, v in med.items()},
-                          sum_median_ms=round(statistics.median(totals), 5), gemms=shapes)))
+    extra = {}
+    if not self_attn:
+        extra["act_ms"] = round(whole_act_ms(pol, obs, h, masks, noise, a.warmup, a.reps), 5)
+        extra["rollout"] = rollout_rate(N, H, dev, a.warmup, a.rollout_steps)
+        print("whole act (profiling off): %.4f ms median" % extra["act_ms"])
+        print("device-resident rollout, CrowdSimPred-v0, N = %d, H = %d: %.3f M env-steps/s (%.4f ms per step)"
+              % (N, H, extra["rollout"]["env_steps_per_s"] / 1e6, extra["rollout"]["ms_per_step"]))
+    print(json.dumps(dict(card=info, N=N, H=H, self_attn=self_attn, rows=rows, reps=a.reps,
+                          median_ms={k: round(v, 5) for k, v in med.items()},
+                          sum_median_ms=round(statistics.median(totals), 5), gemms=shapes, **extra)))
+
+
+def whole_act_ms(pol, obs, h, masks, noise, warmup, reps):
+    """Median of CUDA-event times around single act calls (profiling off)."""
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    out = []
+    for i in range(warmup + reps):
+        e0.record()
+        pol.act(obs, h, masks, noise=noise)
+        e1.record()
+        e1.synchronize()
+        if i >= warmup:
+            out.append(e0.elapsed_time(e1))
+    return statistics.median(out)
+
+
+def rollout_rate(N, H, dev, warmup, steps):
+    """env step + act of the use_self_attn = False policy into the rollout storage, everything on the device
+    (RolloutStorage.rollout_step_zero_copy, as bench.py's value rate); env-steps/s over `steps` timed steps."""
+    from crowdnav_prediction_attngraph_b200.policy import Policy
+    from crowdnav_prediction_attngraph_b200.storage import RolloutStorage
+    from crowdnav_prediction_attngraph_b200.vec_env import CudaCrowdVecEnv
+    T = 30
+    env = CudaCrowdVecEnv(num_envs=N, seed=425, human_num=H, device=dev)
+
+    class Args(object):
+        num_processes, seq_length, num_mini_batch, use_self_attn = N, T, 2, False
+    torch.manual_seed(425)
+    policy = Policy(env.observation_space.spaces, env.action_space, base_kwargs=Args(), base='selfAttn_merge_srnn').to(dev)
+    ro = RolloutStorage(T, N, env.observation_space.spaces, env.action_space, 128, 256, device=dev)
+    obs = env.reset()
+    for k in ro.obs:
+        ro.obs[k][0].copy_(obs[k])
+    eng = policy._engine(N, dev)
+
+    def step():
+        ro.rollout_step_zero_copy(eng, env)
+        if ro.step == 0:
+            ro.after_update()
+    for _ in range(warmup + 400):           # burn-in: episodes desynchronise, as bench.py's --burn-in
+        step()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        step()
+    e1.record()
+    e1.synchronize()
+    ms = e0.elapsed_time(e1) / steps
+    env.close()
+    return dict(env_steps_per_s=round(N / ms * 1e3, 1), ms_per_step=round(ms, 5), steps=steps)
 
 
 if __name__ == "__main__":
