@@ -329,11 +329,16 @@ CN_HD void cn_orca_build(const CnParams& p, const CnState& g, CnEnvSh& s, int e,
 // Social-force humans (humans.policy = 'social_force', crowd_nav/policy/social_force.py:11-49): pull towards the goal
 // with relaxation K_I, exponential push A exp((r_i + r_j - d) / B) from every other human (the ones outside the FOV are
 // replaced by the dummy at (7, 7), crowd_sim.py:680-703), explicit Euler step, speed clipped to v_pref.  fp64 like the
-// reference's Python floats, same expression order.  Writes s.nwx / s.nwy and the robot-collision distance.
+// reference's Python floats, same expression order.
 // VIS (robot.visible): the robot, or outside the FOV the dummy robot at (7, 7), pushes too, radius robot.radius; it is
 // the last term of the sum.
+// cn_sf_velocity is the velocity alone, read from the joint state in s (positions px / py, fp64 velocities wx / wy):
+// it writes nothing, so the test phase's ground-truth look-ahead (use_fov = false: every other human as is, never the
+// robot) calls it on its scratch rows.  cn_sf_action is get_human_actions: it publishes the velocity, the diagnostics
+// and the robot-collision distance.
+struct CnD2 { double x, y; };
 template <bool VIS = false>
-CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h, bool use_fov = true) {
+CN_HD CnD2 cn_sf_velocity(const CnParams& p, const CnEnvSh& s, int h, bool use_fov) {
   const int hn = s.hn;
   const double px = s.px[h], py = s.py[h], vx = s.wx[h], vy = s.wy[h];
   const double dx = s.gx[h] - px, dy = s.gy[h] - py;
@@ -363,6 +368,14 @@ CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, 
   double nvy = vy + (dvy + ivy) * p.time_step;
   const double nrm = cn_norm_dot(nvx, nvy);                  // np.linalg.norm([new_vx, new_vy])
   if (nrm > s.vpref[h]) { nvx = nvx / nrm * s.vpref[h]; nvy = nvy / nrm * s.vpref[h]; }
+  return CnD2{nvx, nvy};
+}
+
+template <bool VIS = false>
+CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h) {
+  const double px = s.px[h], py = s.py[h];
+  const CnD2 v = cn_sf_velocity<VIS>(p, s, h, true);
+  const double nvx = v.x, nvy = v.y;
   s.nwx[h] = nvx; s.nwy[h] = nvy;
   s.nvx[h] = (float)nvx; s.nvy[h] = (float)nvy;
   const size_t i = cn_idx(p, e, h);
@@ -372,7 +385,9 @@ CN_HD void cn_sf_action(const CnParams& p, const CnState& g, CnEnvSh& s, int e, 
 }
 
 // Diagnostics of the LAST ORCA solve of a human's simulator (what reading the reference's rvo2 sims after a
-// step shows; in the test phase that is the final look-ahead solve).
+// step shows; in the test phase that is the final look-ahead solve).  Social-force humans have no simulator: their
+// diagnostics are always the real action of the step (cn_sf_action) with 0 lines and no failure, in phase 'test'
+// too, where the look-ahead's last velocity is not kept (the reference has nothing to read it from).
 CN_HD void cn_orca_diag(const CnParams& p, const CnState& g, int e, int h, CnF2 result, int nl, int fail) {
   const size_t i = cn_idx(p, e, h);
   g.last_hvx[i] = result.x; g.last_hvy[i] = result.y;

@@ -64,6 +64,37 @@ __device__ inline CnEnvSh* env_view(unsigned char* base, const EnvSmemLayout& L,
   return s;
 }
 
+// Ground-truth look-ahead of social-force humans in phase 'test' (crowd_sim_var_num.py:180-206): lookahead_steps fp64
+// SOCIAL_FORCE.predict steps of the humans only (no FOV dummies, never the robot).  The scratch rows are the humans'
+// own px / py / wx / wy in shared memory, and the 'future' danger zone inputs accumulate in t0 / t1 (free in phase
+// 'test': the reward recomputes the collision distance): across a barrier a thread holds nothing but its new velocity.
+// The rows are restored from HBM, which holds them unchanged until cn_phase_store.  The real action (nwx / nwy / nvx /
+// nvy) is not touched.  CTA-uniform call (barriers); `live` = the thread owns a human.
+__device__ __forceinline__ void cn_sf_lookahead(const CnParams& p, const CnState& g, CnEnvSh* s, int e, int h, bool live) {
+  const bool vis_prev = live && g.vis[cn_idx(p, e, h)] != 0;
+  if (live) { s->t0[h] = INFINITY; s->t1[h] = 0.0; }
+  for (int t = 1; t <= p.lookahead_steps; ++t) {
+    __syncthreads();                                                  // row t - 1 complete
+    CnD2 v = {0.0, 0.0};
+    if (live) v = cn_sf_velocity(p, *s, h, false);
+    __syncthreads();                                                  // every read of row t - 1 done
+    if (live) {
+      const double x = s->px[h] + v.x * p.time_step, y = s->py[h] + v.y * p.time_step;   // agent.py:185-192
+      s->px[h] = x; s->py[h] = y; s->wx[h] = v.x; s->wy[h] = v.y;
+      if (t % p.pred_interval == 0) {
+        CnLookahead la; la.min_rd = s->t0[h]; la.pen = s->t1[h];
+        cn_lookahead_accumulate(p, *s, vis_prev, x, y, t / p.pred_interval, la);
+        s->t0[h] = la.min_rd; s->t1[h] = la.pen;                      // reward inputs (test phase)
+      }
+    }
+  }
+  __syncthreads();
+  if (live) {
+    const size_t i = cn_idx(p, e, h);
+    s->px[h] = g.hpx[i]; s->py[h] = g.hpy[i]; s->wx[h] = g.hwx[i]; s->wy[h] = g.hwy[i];
+  }
+}
+
 // One rollout step of every environment.  Episodes that finish INSTALL their prepared successor
 // (g.prep_*, computed off the critical path by cn_env_event_kernel) and emit its first observation in
 // the same launch.  mode 1 = reset of the whole vector env: no step, every environment installs.
@@ -71,7 +102,9 @@ __device__ inline CnEnvSh* env_view(unsigned char* base, const EnvSmemLayout& L,
 // policy's kernel carries none of its code.  VIS: robot_visible != 0 (the humans' solves see the robot), likewise.
 // COLLECT: CrowdSimVarNumCollect-v0 (p.collect): collect reward, prediction ids and the pred_info rows instead of the
 // training observation.  Phase 'train' only (cn_env_create_collect), so it carries no ground-truth look-ahead.
-template <int MAXH, int MAXW, bool ROBOT, bool VIS, bool COLLECT = false>
+// SFLA: social-force humans in phase 'test' (cn_sf_lookahead); its own instantiations, so the kernels of ORCA humans and
+// of phase 'train' carry none of the look-ahead's code.
+template <int MAXH, int MAXW, bool ROBOT, bool VIS, bool COLLECT = false, bool SFLA = false>
 __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState g, const float* __restrict__ action,
                                                           CnObs ob, CnStepOut out, int epb, int line_cap, int mode) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -170,6 +203,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
   };
   if (mode != 1 && p.social_force) {
     if (live) cn_sf_action<VIS>(p, g, *s, e, h);                           // social-force humans: no linear programs
+    if (SFLA) cn_sf_lookahead(p, g, s, e, h, live);                   // phase 'test' (CTA-uniform: barriers)
   } else if (mode == 2) {
     // finishing pass of a step whose ORCA solve already ran on the side stream (mode 3, same state: the humans' solve
     // reads the robot's position and velocity as the previous step left them, never this step's action)
@@ -515,8 +549,17 @@ KernelFn pick_kernel_collect(int maxh) {
   return cn_env_step_kernel<128, 16, true, true, true>;
 }
 
-KernelFn pick_kernel(int maxh, bool robot, bool vis, bool collect = false) {
-  if (collect) return pick_kernel_collect(maxh);
+// social-force humans in phase 'test' (the SF look-ahead): robot policy and visibility stay run-time parameters too
+KernelFn pick_kernel_sfla(int maxh) {
+  if (maxh <= 32) return cn_env_step_kernel<32, 16, true, true, false, true>;
+  if (maxh <= 64) return cn_env_step_kernel<64, 16, true, true, false, true>;
+  return cn_env_step_kernel<128, 16, true, true, false, true>;
+}
+
+KernelFn pick_kernel(const CnParams& p, int maxh) {
+  if (p.collect) return pick_kernel_collect(maxh);
+  if (p.social_force && p.test_phase) return pick_kernel_sfla(maxh);
+  const bool robot = p.robot_policy != 0, vis = p.robot_visible != 0;
   return vis ? pick_kernel_vis<true>(maxh, robot) : pick_kernel_vis<false>(maxh, robot);
 }
 
@@ -578,7 +621,7 @@ int launch_step(cn_env* env, const float* d_action, const cn_obs_ptrs* o, const 
     env->prep_dirty = false;
   }
   const int grid = (env->p.N + env->epb - 1) / env->epb;
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0, env->p.collect != 0);
+  KernelFn fn = pick_kernel(env->p, env->maxh);
   CnObs ob = to_obs(o);
   ob.pred_info = d_pred_info;
   // mode 0 with a pre-solve of this state done on the side stream (joined above) -> finishing pass only (mode 2)
@@ -701,11 +744,6 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
     cn_env_destroy(env);
     return cn_set_error("cn_env_create: human_policy %d unsupported (0 = 'orca', 1 = 'social_force')", cfg->human_policy);
   }
-  if (cfg->human_policy == 1 && cfg->phase == 2) {
-    cn_env_destroy(env);
-    return cn_set_error("cn_env_create: social-force humans are covered in phase 'train' only (the test phase's "
-                        "ground-truth look-ahead runs the ORCA solver)");
-  }
   if (cfg->robot_policy < 0 || cfg->robot_policy > 2) {
     cn_env_destroy(env);
     return cn_set_error("cn_env_create: robot_policy %d unsupported (0 = the caller's action, 1 = 'orca', 2 = 'social_force')",
@@ -814,7 +852,7 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
   const EnvSmemLayout L = env_layout(p.H, true, p.social_force != 0);
   int nsm = 0;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-  KernelFn fn = pick_kernel(env->maxh, env->p.robot_policy != 0, env->p.robot_visible != 0, collect);
+  KernelFn fn = pick_kernel(p, env->maxh);
   // dynamic shared memory: 227 KiB less the kernel's static part (the collect instantiation's ballot words)
   size_t smem_cap = 227 * 1024;
   {

@@ -94,6 +94,28 @@ CASES = {
     "env_varnum_h10_vis_fov1": dict(env_name="CrowdSimVarNum-v0", human_num=10, predict_method="none",
                                     robot_visible=True, human_fov=1.0, randomize=True, goal_changing=True, nenv=3,
                                     steps=200, seed=17),
+    # social-force humans in phase 'test': the ground-truth look-ahead runs SOCIAL_FORCE.predict on the humans only (no
+    # FOV dummies, never the robot, fp64 rows), every pred_interval-th row feeds the 'future' danger zone and, on
+    # CrowdSimPred-v0, the future-collision penalty
+    "env_varnum_h8_sf_test_rand": dict(env_name="CrowdSimVarNum-v0", human_num=8, predict_method="none",
+                                       human_policy="social_force", randomize=True, goal_changing=True, nenv=2,
+                                       steps=160, seed=21, phase="test"),
+    "env_pred_h10_sf_test_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="const_vel",
+                                      human_policy="social_force", randomize=True, goal_changing=True, nenv=2,
+                                      steps=200, seed=11, phase="test"),
+    "env_varnum_h8_sf_test_vis_rand": dict(env_name="CrowdSimVarNum-v0", human_num=8, predict_method="none",
+                                           human_policy="social_force", robot_visible=True, randomize=True,
+                                           goal_changing=True, nenv=2, steps=160, seed=21, phase="test"),
+    "env_varnum_h6_range2_sf_test": dict(env_name="CrowdSimVarNum-v0", human_num=6, predict_method="none",
+                                         human_num_range=2, human_policy="social_force", randomize=True,
+                                         goal_changing=True, nenv=3, steps=200, seed=9, phase="test"),
+    "env_varnum_h20_test_sf_humans_orca_robot": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                                     human_policy="social_force", robot_policy="orca", randomize=False,
+                                                     goal_changing=False, nenv=2, steps=120, seed=425, phase="test"),
+    "env_varnum_h20_test_sf_humans_sf_robot": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                                   human_policy="social_force", robot_policy="social_force",
+                                                   randomize=False, goal_changing=False, nenv=2, steps=120, seed=425,
+                                                   phase="test"),
 }
 
 

@@ -11,7 +11,11 @@ robot position ends the path (rl/evaluation.py:96-97).  The robot's rvo2 simulat
 the reference; without randomised attributes its frozen parameters are the configured constants, so the split does
 not change them.  Output: tests/golden/eval_baselines.npz.
 
-    python tools/make_golden_eval_baselines.py [--procs 8]
+--humans social_force runs the same protocol among social-force humans (humans.policy = 'social_force', whose phase
+'test' look-ahead runs SOCIAL_FORCE.predict) and writes tests/golden/eval_baselines_sf_humans.npz; the default, orca,
+writes eval_baselines.npz as before.
+
+    python tools/make_golden_eval_baselines.py [--procs 8] [--humans orca|social_force]
 """
 import argparse
 import multiprocessing as mp
@@ -31,7 +35,7 @@ INFO_CODE = {"Timeout": 1, "Collision": 2, "ReachGoal": 3}
 
 
 def run_block(args):
-    policy, lo, hi = args
+    policy, humans, lo, hi = args
     sys.path.insert(0, REF)
     sys.argv = ["x", "--no-cuda", "--env-name", "CrowdSimVarNum-v0"]
     import gym
@@ -40,6 +44,7 @@ def run_block(args):
     from crowd_sim.envs.utils.info import Danger
     cfg = Config()
     cfg.robot.policy = policy
+    cfg.humans.policy = humans
     cfg.sim.human_num = HUMANS
     cfg.sim.predict_method = "none"
     cfg.env.randomize_attributes = False
@@ -76,12 +81,13 @@ def run_block(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--procs", type=int, default=8)
+    ap.add_argument("--humans", choices=("orca", "social_force"), default="orca")
     a = ap.parse_args()
     rec = {}
     with mp.get_context("spawn").Pool(a.procs) as pool:
         for name, policy in BASELINES.items():
             edges = np.linspace(0, TEST_SIZE, 4 * a.procs + 1).astype(int)
-            rows = [r for block in pool.map(run_block, [(policy, lo, hi) for lo, hi in zip(edges[:-1], edges[1:])])
+            rows = [r for block in pool.map(run_block, [(policy, a.humans, lo, hi) for lo, hi in zip(edges[:-1], edges[1:])])
                     for r in block]
             rows.sort()
             rec[name + "_code"] = np.array([r[1] for r in rows], np.int32)
@@ -93,7 +99,8 @@ def main():
             rec[name + "_min_dist"] = np.array([x for r in rows for x in r[5]])
             codes = rec[name + "_code"]
             print(name, "success %.2f collision %.2f timeout %.2f" % tuple(np.mean(codes == c) for c in (3, 2, 1)))
-    path = os.path.join(REPO, "tests", "golden", "eval_baselines.npz")
+    fname = "eval_baselines.npz" if a.humans == "orca" else "eval_baselines_sf_humans.npz"
+    path = os.path.join(REPO, "tests", "golden", fname)
     np.savez_compressed(path, **rec)
     print("wrote", path, os.path.getsize(path) // 1024, "KiB")
 
