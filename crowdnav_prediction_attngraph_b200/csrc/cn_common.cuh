@@ -29,7 +29,7 @@ struct CnParams {
   int hbase;        // sim.human_num
   int P;            // sim.predict_steps
   int W;            // spatial_edges row width: 2*(P+1) (CrowdSimPred) or 2 (CrowdSimVarNum)
-  int const_vel;    // 1: CrowdSimPred-v0 'const_vel'; 0: CrowdSimVarNum-v0 'none'
+  int const_vel;    // 1: CrowdSimPred-v0 'const_vel'; 2: CrowdSimPred-v0 'truth'; 0: CrowdSimVarNum-v0 'none'
   int randomize;    // env.randomize_attributes
   int goal_changing;      // humans.random_goal_changing
   int end_goal_changing;  // humans.end_goal_changing

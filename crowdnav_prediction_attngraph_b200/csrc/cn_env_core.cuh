@@ -414,6 +414,19 @@ CN_HD void cn_lookahead_accumulate(const CnParams& p, const CnEnvSh& s, bool vis
   }
 }
 
+// generate_ob with sim.predict_method = 'truth' (crowd_sim_pred.py:80-90): kept look-ahead position k (1-based) of a
+// human the robot sees, relative to the robot's position after the step, as observation columns 2k, 2k + 1 (fp64
+// difference narrowed to fp32), and the future-collision penalty the next step's reward reads
+// (CrowdSimPred.calc_reward, crowd_sim_pred.py:216-233): the test of the 'const_vel' rows in cn_phase_obs_a.
+CN_HD void cn_truth_row(const CnParams& p, const CnEnvSh& s, double x, double y, int k, float* row, double& pen) {
+  const double rx = x - s.rpx, ry = y - s.rpy;
+  row[2 * k] = (float)rx; row[2 * k + 1] = (float)ry;
+  double coef = 2.0;
+  for (int q = 0; q < k; ++q) coef = coef * 2.0;              // 2^(k+1)
+  const double c = (cn_norm_plain(rx, ry) < p.robot_radius + p.human_radius) ? (p.collision_penalty / coef) : 0.0;
+  pen = c < pen ? c : pen;
+}
+
 // Phase ORCA, part 3 (per thread): publish the solved velocity + the robot-collision distance.
 CN_HD void cn_orca_finish(const CnParams& p, const CnState& g, CnEnvSh& s, int e, int h, CnF2 result, int nl, int fail) {
   const size_t i = cn_idx(p, e, h);

@@ -95,6 +95,33 @@ __device__ __forceinline__ void cn_sf_lookahead(const CnParams& p, const CnState
   }
 }
 
+// Observation look-ahead of social-force humans with sim.predict_method = 'truth' (generate_ob ->
+// calc_human_future_traj('truth')): the steps of cn_sf_lookahead from the state after this step (integrated, humans
+// joined / left, episodes installed), whose rows are not in HBM yet, so each thread keeps its own human's row in
+// registers and puts it back.  Every pred_interval-th row of a human the robot sees goes into its observation row and
+// the future-collision penalty t1 (cn_truth_row); t0 (cn_phase_obs_a's sort key) is untouched.  CTA-uniform call.
+__device__ __forceinline__ void cn_sf_obs_lookahead(const CnParams& p, CnEnvSh* s, int h, bool live, float* row) {
+  const bool seen = live && s->visr[h] != 0;
+  double spx = 0.0, spy = 0.0, swx = 0.0, swy = 0.0, pen = 0.0;
+  if (live) { spx = s->px[h]; spy = s->py[h]; swx = s->wx[h]; swy = s->wy[h]; }
+  for (int t = 1; t <= p.lookahead_steps; ++t) {
+    __syncthreads();                                                  // row t - 1 complete
+    CnD2 v = {0.0, 0.0};
+    if (live) v = cn_sf_velocity(p, *s, h, false);
+    __syncthreads();                                                  // every read of row t - 1 done
+    if (live) {
+      const double x = s->px[h] + v.x * p.time_step, y = s->py[h] + v.y * p.time_step;
+      s->px[h] = x; s->py[h] = y; s->wx[h] = v.x; s->wy[h] = v.y;
+      if (seen && t % p.pred_interval == 0) cn_truth_row(p, *s, x, y, t / p.pred_interval, row, pen);
+    }
+  }
+  __syncthreads();
+  if (live) {
+    s->px[h] = spx; s->py[h] = spy; s->wx[h] = swx; s->wy[h] = swy;
+    if (seen) s->t1[h] = pen;
+  }
+}
+
 // One rollout step of every environment.  Episodes that finish INSTALL their prepared successor
 // (g.prep_*, computed off the critical path by cn_env_event_kernel) and emit its first observation in
 // the same launch.  mode 1 = reset of the whole vector env: no step, every environment installs.
@@ -104,7 +131,11 @@ __device__ __forceinline__ void cn_sf_lookahead(const CnParams& p, const CnState
 // training observation.  Phase 'train' only (cn_env_create_collect), so it carries no ground-truth look-ahead.
 // SFLA: social-force humans in phase 'test' (cn_sf_lookahead); its own instantiations, so the kernels of ORCA humans and
 // of phase 'train' carry none of the look-ahead's code.
-template <int MAXH, int MAXW, bool ROBOT, bool VIS, bool COLLECT = false, bool SFLA = false>
+// TRUTH: CrowdSimPred-v0 with sim.predict_method = 'truth' (p.const_vel 2): every observation runs the ground-truth
+// look-ahead and observes its rows, ORCA humans (SFLA false) or social-force humans (SFLA true, whose phase-'test'
+// look-ahead then runs in phase 'test' only).  Robot policy 0; robot visibility is a run-time parameter (VIS true), which
+// also makes a simulator the look-ahead creates freeze every human's true radius (cn_orca_build).
+template <int MAXH, int MAXW, bool ROBOT, bool VIS, bool COLLECT = false, bool SFLA = false, bool TRUTH = false>
 __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState g, const float* __restrict__ action,
                                                           CnObs ob, CnStepOut out, int epb, int line_cap, int mode) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -157,19 +188,19 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
   __syncthreads();
   // live = this thread's slot holds a human (slots [hn, H) are empty when sim.human_num_range > 0)
   const bool live = active && h < s->hn;
-  // One ORCA solve of every human of the CTA on the joint state currently in shared memory (CTA-uniform
-  // call: contains barriers).  linearProgram3 (needed by ~30 % of the humans in steady state) is
-  // balanced across the whole CTA: failed humans are queued in shared memory and every warp pops tasks
-  // until the queue is dry.
+  // One ORCA solve of every human of the CTA on the joint state currently in shared memory (CTA-uniform call: contains
+  // barriers; `lv` = this thread's slot holds a human).  linearProgram3 (needed by ~30 % of the humans in steady state)
+  // is balanced across the whole CTA: failed humans are queued in shared memory and every warp pops tasks until the
+  // queue is dry.
   int* lp3_count = reinterpret_cast<int*>(lp3_q);
   int* lp3_head = lp3_count + 1;
   unsigned short* lp3_tasks = reinterpret_cast<unsigned short*>(lp3_count + 2);
-  auto orca_solve = [&](bool use_fov, CnF2& result, int& nl, int& fail) {
+  auto orca_solve = [&](bool lv, bool use_fov, CnF2& result, int& nl, int& fail) {
     nl = 0; fail = -1;
     float vmax = 0.0f;
     CnF2 pref = f2(0.0f, 0.0f);
     result = f2(0.0f, 0.0f);
-    if (live) cn_orca_build<MAXH, VIS>(p, g, *s, e, h, W.of(lane), nl, vmax, pref, use_fov, mode == 3 ? (uint8_t)2 : (uint8_t)1);
+    if (lv) cn_orca_build<MAXH, VIS>(p, g, *s, e, h, W.of(lane), nl, vmax, pref, use_fov, mode == 3 ? (uint8_t)2 : (uint8_t)1);
     __syncwarp();
     cn_orca_lp2_warp(hco, W, nl, vmax, pref, result, fail);           // per half-warp; idle lanes with nl = 0
     if (fail >= 0) {
@@ -203,7 +234,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
   };
   if (mode != 1 && p.social_force) {
     if (live) cn_sf_action<VIS>(p, g, *s, e, h);                           // social-force humans: no linear programs
-    if (SFLA) cn_sf_lookahead(p, g, s, e, h, live);                   // phase 'test' (CTA-uniform: barriers)
+    if (SFLA && (!TRUTH || p.test_phase)) cn_sf_lookahead(p, g, s, e, h, live);   // phase 'test' (CTA-uniform: barriers)
   } else if (mode == 2) {
     // finishing pass of a step whose ORCA solve already ran on the side stream (mode 3, same state: the humans' solve
     // reads the robot's position and velocity as the previous step left them, never this step's action)
@@ -215,7 +246,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
     }
   } else if (mode != 1) {
     CnF2 result; int nl, fail;
-    orca_solve(true, result, nl, fail);                               // get_human_actions (crowd_sim.py:680-703)
+    orca_solve(live, true, result, nl, fail);                         // get_human_actions (crowd_sim.py:680-703)
     if (live && fail >= 0) atomicAdd(&s->lp3_cost, 1);              // cost estimate for the next step's balancing
     if (mode == 3) {                                                  // pre-solve: publish the result and stop
       if (live) {
@@ -246,7 +277,7 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
           s->px[h] = lx; s->py[h] = ly; s->fx[h] = (float)lx; s->fy[h] = (float)ly; s->vx[h] = lvx; s->vy[h] = lvy;
         }
         __syncthreads();
-        orca_solve(false, lres, lnl, lfail);
+        orca_solve(live, false, lres, lnl, lfail);
         lx = lx + (double)lres.x * p.time_step; ly = ly + (double)lres.y * p.time_step;
         lvx = lres.x; lvy = lres.y;
         if (live && t % p.pred_interval == 0) cn_lookahead_accumulate(p, *s, vis_prev, lx, ly, t / p.pred_interval, la);
@@ -307,6 +338,51 @@ __global__ void __launch_bounds__(288, 2) cn_env_step_kernel(CnParams p, CnState
   }
   if (active) cn_phase_obs_a<MAXW>(p, g, *s, e, h, row);
   __syncthreads();
+  if (TRUTH) {
+    // generate_ob with sim.predict_method = 'truth' (crowd_sim_pred.py:62-97): after the visibility and belief update
+    // (cn_phase_obs_a, whose row holds the k = 0 columns and the sort key) calc_human_future_traj('truth') runs
+    // lookahead_steps nested solves of the live humans from their true state after this step: humans joined / left
+    // and installed episodes included, so liveness is taken from the current count.  The rows of the humans the
+    // robot sees (visibility of this observation) replace the 'const_vel' columns 2.. and the penalty t1; the others
+    // keep cn_phase_obs_a's (15, 15) penalty and are written as 15 by cn_phase_obs_b.
+    const bool olive = active && h < s->hn;
+    if (SFLA) {
+      cn_sf_obs_lookahead(p, s, h, olive, row);
+    } else {
+      // ORCA humans: the solves go through each human's cached simulator (orca_solve, use_fov = false: every other human
+      // as is, never the robot), creating it when missing or when the agent count changed; every thread keeps its own
+      // human's row and the sort key (the LP3 queue borrows t0) in registers.  The last solve is the simulator's
+      // diagnostics (cn_orca_diag).  The loop is the test phase's above, written out again: one loop shared by both
+      // changes the instruction schedule of the instantiations without TRUTH.
+      const bool seen = olive && s->visr[h] != 0;
+      double spx = 0, spy = 0, lx = 0, ly = 0, key = 0, pen = 0.0;
+      float svx = 0, svy = 0, lvx = 0, lvy = 0;
+      if (olive) {
+        spx = s->px[h]; spy = s->py[h]; svx = s->vx[h]; svy = s->vy[h]; key = s->t0[h];
+        lx = spx; ly = spy; lvx = svx; lvy = svy;
+      }
+      CnF2 lres = f2(0.0f, 0.0f); int lnl = 0, lfail = -1;
+      for (int t = 1; t <= p.lookahead_steps; ++t) {
+        __syncthreads();
+        if (olive) {
+          s->px[h] = lx; s->py[h] = ly; s->fx[h] = (float)lx; s->fy[h] = (float)ly; s->vx[h] = lvx; s->vy[h] = lvy;
+        }
+        __syncthreads();
+        orca_solve(olive, false, lres, lnl, lfail);
+        lx = lx + (double)lres.x * p.time_step; ly = ly + (double)lres.y * p.time_step;
+        lvx = lres.x; lvy = lres.y;
+        if (seen && t % p.pred_interval == 0) cn_truth_row(p, *s, lx, ly, t / p.pred_interval, row, pen);
+      }
+      __syncthreads();
+      if (olive) {
+        s->px[h] = spx; s->py[h] = spy; s->fx[h] = (float)spx; s->fy[h] = (float)spy; s->vx[h] = svx; s->vy[h] = svy;
+        s->t0[h] = key;
+        if (seen) s->t1[h] = pen;
+        if (p.lookahead_steps > 0) cn_orca_diag(p, g, e, h, lres, lnl, lfail);
+      }
+    }
+    __syncthreads();
+  }
   if (active) cn_phase_obs_b(p, g, *s, e, h, row, ob);
   __syncthreads();
   if (active) {
@@ -556,8 +632,18 @@ KernelFn pick_kernel_sfla(int maxh) {
   return cn_env_step_kernel<128, 16, true, true, false, true>;
 }
 
+// CrowdSimPred-v0 with sim.predict_method = 'truth' (the observation look-ahead): ORCA or social-force humans, robot
+// visibility a run-time parameter, robot policy 0
+template <bool SF>
+KernelFn pick_kernel_truth(int maxh) {
+  if (maxh <= 32) return cn_env_step_kernel<32, 16, false, true, false, SF, true>;
+  if (maxh <= 64) return cn_env_step_kernel<64, 16, false, true, false, SF, true>;
+  return cn_env_step_kernel<128, 16, false, true, false, SF, true>;
+}
+
 KernelFn pick_kernel(const CnParams& p, int maxh) {
   if (p.collect) return pick_kernel_collect(maxh);
+  if (p.const_vel == 2) return p.social_force ? pick_kernel_truth<true>(maxh) : pick_kernel_truth<false>(maxh);
   if (p.social_force && p.test_phase) return pick_kernel_sfla(maxh);
   const bool robot = p.robot_policy != 0, vis = p.robot_visible != 0;
   return vis ? pick_kernel_vis<true>(maxh, robot) : pick_kernel_vis<false>(maxh, robot);
@@ -681,6 +767,9 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
       cfg->human_num + cfg->human_num_range > 128)
     return cn_set_error("cn_env_create: need num_envs > 0, 0 <= human_num_range < human_num and human_num + range <= 128 "
                         "(got %d, %d, %d)", cfg->num_envs, cfg->human_num, cfg->human_num_range);
+  if (cfg->const_vel < 0 || cfg->const_vel > 2)
+    return cn_set_error("cn_env_create: const_vel %d unsupported (0 = CrowdSimVarNum-v0, 1 = CrowdSimPred-v0 'const_vel', "
+                        "2 = CrowdSimPred-v0 'truth')", cfg->const_vel);
   if (cfg->const_vel && (cfg->predict_steps < 0 || 2 * (cfg->predict_steps + 1) > 16))
     return cn_set_error("cn_env_create: predict_steps %d unsupported (row width > 16)", cfg->predict_steps);
   {
@@ -712,13 +801,14 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
     const char* ns = getenv("CN_NO_SIDE_STREAM");       // debugging / profiling aid
     env->use_side = !(ns && ns[0] == '1');
     // pre-solve of the next step's ORCA on the side stream (launch_step).  Not with social-force humans (no linear
-    // programs to move) nor in the test phase (its look-ahead solves stay with the step).  Default: on for crowds of up
+    // programs to move) nor in the test phase (its look-ahead solves stay with the step) nor with 'truth' predictions (the
+    // observation look-ahead creates simulators, which the pre-solve's provisional marks do not cover).  Default: on for crowds of up
     // to 32 human slots (measured: 20 humans 0.455 -> 0.442 ms/step, e2e 0.534 -> 0.501), off above (50 humans 2.15 ->
     // 2.19, 100 humans 4.9 -> 5.1 ms/step: the many short CTAs of the large-H solve take SMs from the policy's GEMMs
     // instead of filling gaps); CN_PRESOLVE=1 / 0 forces it.
     const char* ps = getenv("CN_PRESOLVE");
     const bool want = ps ? ps[0] != '0' : (cfg->human_num + cfg->human_num_range <= 32);
-    env->presolve = env->use_side && want && cfg->human_policy == 0 && cfg->phase != 2;
+    env->presolve = env->use_side && want && cfg->human_policy == 0 && cfg->phase != 2 && cfg->const_vel != 2;
     env->presolved = false;
   }
   err = cudaStreamCreateWithFlags(&env->side, cudaStreamNonBlocking);
@@ -729,7 +819,7 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
   memset(&p, 0, sizeof(p));
   p.hbase = cfg->human_num; p.hrange = cfg->human_num_range;
   p.N = cfg->num_envs; p.H = cfg->human_num + cfg->human_num_range; p.P = cfg->predict_steps;
-  p.const_vel = cfg->const_vel ? 1 : 0;
+  p.const_vel = cfg->const_vel;                 // 0, 1 or 2 ('truth': the TRUTH instantiations, pick_kernel)
   p.W = p.const_vel ? 2 * (p.P + 1) : 2;
   p.randomize = cfg->randomize_attributes; p.goal_changing = cfg->random_goal_changing;
   p.end_goal_changing = cfg->end_goal_changing; p.sort_humans = cfg->sort_humans;
@@ -758,11 +848,12 @@ int env_create(const cn_config* cfg, cn_env** out, bool collect) {
     cn_env_destroy(env);
     return cn_set_error("cn_env_create: robot_visible %d unsupported (0 or 1)", cfg->robot_visible);
   }
-  if (cfg->robot_visible && cfg->const_vel) {
+  if (cfg->robot_visible && cfg->const_vel == 1) {
     cn_env_destroy(env);
-    return cn_set_error("cn_env_create: robot_visible is covered for CrowdSimVarNum-v0 (const_vel 0) only: the reference's "
-                        "CrowdSimPred-v0 cannot run it (calc_human_future_traj('const_vel') assigns the humans' (H, 2) "
-                        "velocities into an (H + 1, 2) slice and raises on the first reset)");
+    return cn_set_error("cn_env_create: robot_visible is covered for CrowdSimVarNum-v0 (const_vel 0) and 'truth' (const_vel "
+                        "2) only: the reference's CrowdSimPred-v0 with 'const_vel' cannot run it "
+                        "(calc_human_future_traj('const_vel') assigns the humans' (H, 2) velocities into an (H + 1, 2) "
+                        "slice and raises on the first reset)");
   }
   if (cfg->phase != 0 && cfg->phase != 2) {
     cn_env_destroy(env);

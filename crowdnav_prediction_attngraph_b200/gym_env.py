@@ -139,7 +139,8 @@ class _GymCrowdEnv(object):
 
 
 class CrowdSimPred(_GymCrowdEnv):
-    """crowd_sim/envs/crowd_sim_pred.py (predict_method 'const_vel')."""
+    """crowd_sim/envs/crowd_sim_pred.py, with sim.predict_method 'const_vel' (constant-velocity predictions) or 'truth'
+    (every observation runs the ground-truth look-ahead; robot.visible = True is covered there)."""
     _engine_id = "CrowdSimPred-v0"
 
 

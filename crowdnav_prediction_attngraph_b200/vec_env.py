@@ -83,6 +83,8 @@ class Box(_Space):
 
 # robot.policy -> cn_config.robot_policy (0: the caller's action)
 ROBOT_POLICIES = {"orca": 1, "social_force": 2}
+# sim.predict_method on CrowdSimPred-v0 -> cn_config.const_vel
+PREDICT_METHODS = {"const_vel": 1, "truth": 2}
 COLLECT_ENV = "CrowdSimVarNumCollect-v0"
 
 
@@ -120,15 +122,20 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
     if config.humans.policy not in ("orca", "social_force"):
         raise NotImplementedError("humans.policy %r: the engine covers 'orca' and 'social_force'" % (config.humans.policy,))
     if env_name == "CrowdSimPred-v0":
-        if config.sim.predict_method != "const_vel":
-            raise NotImplementedError("CrowdSimPred-v0 is covered for predict_method='const_vel'")
-        const_vel = 1
+        # cn_config.const_vel: 1 = constant-velocity predictions, 2 = the ground-truth look-ahead's (arguments.py:195-197)
+        if config.sim.predict_method not in PREDICT_METHODS:
+            raise NotImplementedError("CrowdSimPred-v0 is covered for predict_method 'const_vel' and 'truth' (got %r)"
+                                      % (config.sim.predict_method,))
+        const_vel = PREDICT_METHODS[config.sim.predict_method]
     elif env_name in ("CrowdSimVarNum-v0", COLLECT_ENV):
+        if env_name == COLLECT_ENV and config.sim.predict_method == "truth":
+            raise NotImplementedError("sim.predict_method='truth' is covered on CrowdSimPred-v0 only, not on "
+                                      "CrowdSimVarNumCollect-v0")
         const_vel = 0
     else:
         raise NotImplementedError("env id %r is not covered by the CUDA engine" % env_name)
     robot_visible = bool(config.robot.visible)
-    if robot_visible and const_vel:
+    if robot_visible and const_vel == 1:
         raise NotImplementedError(
             "robot.visible=True on CrowdSimPred-v0 is not covered: the reference cannot run it (calc_human_future_traj("
             "'const_vel') assigns prev_human_pos[:, 2:4], shape (H, 2), into an (H + 1, 2) slice, crowd_sim_var_num.py:"
@@ -456,6 +463,9 @@ def make_vec_envs(env_name, seed, num_processes, gamma, log_dir, device, allow_e
     `phase=` overrides (batched evaluation)."""
     device = torch.device(device)
     if pretext_wrapper or env_name == "CrowdSimPredRealGST-v0":
+        if config is not None and config.sim.predict_method == "truth":
+            raise NotImplementedError("sim.predict_method='truth' is covered on CrowdSimPred-v0 only, not behind the GST "
+                                      "wrapper (pretext_wrapper=True / CrowdSimPredRealGST-v0)")
         if gst_params is None:
             raise ValueError("CrowdSimPredRealGST-v0 / pretext_wrapper=True needs gst_params= (the predictor checkpoint's "
                              "model_state_dict, config.pred.model_dir/checkpoint/epoch_100.pt)")

@@ -48,7 +48,9 @@ typedef struct cn_config {
   int32_t seed;              /* --seed (arguments.py:47)                                        */
   int32_t human_num;         /* sim.human_num                                                    */
   int32_t predict_steps;     /* sim.predict_steps                                               */
-  int32_t const_vel;         /* 1: CrowdSimPred-v0 / 'const_vel'; 0: CrowdSimVarNum-v0 / 'none' */
+  int32_t const_vel;         /* 1: CrowdSimPred-v0 / 'const_vel'; 2: CrowdSimPred-v0 / 'truth' (every observation runs
+                              * the ground-truth look-ahead and observes its kept rows, crowd_sim_pred.py:62-97; same
+                              * 2 (predict_steps + 1)-wide rows as 1); 0: CrowdSimVarNum-v0 / 'none'               */
   int32_t randomize_attributes;   /* env.randomize_attributes                                   */
   int32_t random_goal_changing;   /* humans.random_goal_changing                                */
   int32_t end_goal_changing;      /* humans.end_goal_changing                                   */
@@ -65,9 +67,10 @@ typedef struct cn_config {
                                    * (crowd_sim_var_num.py:371-377); CrowdSimVarNum-v0 with human_num_range 0 only */
   int16_t robot_visible;          /* robot.visible: 1 = every human's ORCA / social-force solve sees the robot (or, outside
                                    * the human's FOV, the dummy robot at (7, 7)) as one more agent (crowd_sim.py:695-699);
-                                   * CrowdSimVarNum-v0 only.  robot_policy and robot_visible share the 4 bytes robot_policy
-                                   * had as an int32, so the struct keeps its size and every offset (little-endian: a caller
-                                   * that stores robot_policy as an int32 below 32768 leaves robot_visible 0)          */
+                                   * CrowdSimVarNum-v0 and 'truth' (const_vel 0 or 2).  robot_policy and robot_visible
+                                   * share the 4 bytes robot_policy had as an int32, so the struct keeps its size and every
+                                   * offset (little-endian: a caller that stores robot_policy as an int32 below 32768
+                                   * leaves robot_visible 0)                                                          */
   double time_step, time_limit, pred_timestep;
   double circle_radius, arena_size;
   double discomfort_dist, discomfort_penalty_factor, success_reward, collision_penalty;

@@ -116,6 +116,29 @@ CASES = {
                                                    human_policy="social_force", robot_policy="social_force",
                                                    randomize=False, goal_changing=False, nenv=2, steps=120, seed=425,
                                                    phase="test"),
+    # CrowdSimPred-v0 with sim.predict_method = 'truth': every generate_ob (reset included) runs the ground-truth
+    # look-ahead and observes its kept rows; the look-ahead is often the call that creates a human's rvo2 simulator
+    # (after a reset, a join / leave, and with robot.visible on every step), freezing every human's true radius
+    "env_pred_h20_truth": dict(env_name="CrowdSimPred-v0", human_num=20, predict_method="truth", randomize=False,
+                               goal_changing=False, nenv=3, steps=175, seed=425, traj_every=4),
+    "env_pred_h10_truth_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="truth", randomize=True,
+                                    goal_changing=True, nenv=2, steps=200, seed=11),
+    "env_pred_h10_truth_test_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="truth",
+                                         randomize=True, goal_changing=True, nenv=2, steps=200, seed=11, phase="test"),
+    "env_pred_h6_range3_truth": dict(env_name="CrowdSimPred-v0", human_num=6, predict_method="truth", human_num_range=3,
+                                     randomize=True, goal_changing=True, nenv=2, steps=200, seed=9),
+    "env_pred_h10_truth_vis_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="truth",
+                                        robot_visible=True, human_fov=1.0, randomize=True, goal_changing=True, nenv=3,
+                                        steps=200, seed=17),
+    "env_pred_h10_truth_test_vis_rand": dict(env_name="CrowdSimPred-v0", human_num=10, predict_method="truth",
+                                             robot_visible=True, randomize=True, goal_changing=True, nenv=2, steps=200,
+                                             seed=11, phase="test"),
+    "env_pred_h8_sf_truth_rand": dict(env_name="CrowdSimPred-v0", human_num=8, predict_method="truth",
+                                      human_policy="social_force", randomize=True, goal_changing=True, nenv=2,
+                                      steps=160, seed=21),
+    "env_pred_h8_sf_truth_test_rand": dict(env_name="CrowdSimPred-v0", human_num=8, predict_method="truth",
+                                           human_policy="social_force", randomize=True, goal_changing=True, nenv=2,
+                                           steps=160, seed=21, phase="test"),
 }
 
 
@@ -208,7 +231,7 @@ def run_case(name, case):
     import rvo2
     rvo2.ONLY_AGENT0 = False          # the genuine full doStep of every per-human simulator
     H = case["human_num"] + case.get("human_num_range", 0)          # array width = max_human_num
-    W = 12 if case["predict_method"] == "const_vel" else 2
+    W = 12 if case["predict_method"] in ("const_vel", "truth") else 2
     N, T = case["nenv"], case["steps"]
     mode = ["goal", "goal", "rand", "idle"]
     rec = dict(actions=np.zeros((T, N, 2), np.float32), reward=np.zeros((T, N)), done=np.zeros((T, N), bool),
