@@ -40,13 +40,14 @@ class CnCopySeg(C.Structure):
 
 class CnPolicyConfig(C.Structure):
     _fields_ = [("num_envs", C.c_int32), ("human_num", C.c_int32), ("input_size", C.c_int32),
-                ("device", C.c_int32), ("gemm_mode", C.c_int32), ("no_self_attn", C.c_int32)]
+                ("device", C.c_int32), ("gemm_mode", C.c_int32), ("no_self_attn", C.c_int32),
+                ("visible_masks", C.c_int32)]
 
 
 class CnActPtrs(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in (
         "robot_node", "temporal_edges", "spatial_edges", "detected_human_num", "h_in", "masks", "noise",
-        "value", "action", "log_prob", "h_out", "action_mean")]
+        "value", "action", "log_prob", "h_out", "action_mean", "visible_masks")]
 
 
 class CnDsrnnConfig(C.Structure):
@@ -67,7 +68,8 @@ EXPORTS = [
     "cn_env_step_host", "cn_env_state_bytes", "cn_env_state_copy", "cn_env_launch_count", "cn_env_profile", "cn_env_stage_ms",
     "cn_policy_create", "cn_policy_destroy", "cn_policy_set_param", "cn_policy_finalize",
     "cn_policy_act", "cn_policy_launch_count", "cn_policy_last_rows", "cn_policy_profile", "cn_policy_stage_count",
-    "cn_policy_stage_name", "cn_policy_handle_stage_name", "cn_policy_stage_ms", "cn_copy_segments", "cn_fetch_sync",
+    "cn_policy_stage_name", "cn_policy_handle_stage_name", "cn_policy_handle_stage_count", "cn_policy_stage_ms",
+    "cn_copy_segments", "cn_fetch_sync",
     "cn_gst_create", "cn_gst_destroy", "cn_gst_set_param", "cn_gst_finalize", "cn_gst_reset", "cn_gst_step",
     "cn_gst_launch_count",
     "cn_update_linear_saved_bytes", "cn_update_linear_ws_bytes", "cn_update_linear_fwd", "cn_update_linear_bwd",
@@ -168,6 +170,8 @@ def load_library(path=None):
     lib.cn_policy_stage_name.argtypes = [C.c_int]
     lib.cn_policy_handle_stage_name.restype = C.c_char_p
     lib.cn_policy_handle_stage_name.argtypes = [C.c_void_p, C.c_int]
+    lib.cn_policy_handle_stage_count.restype = C.c_int
+    lib.cn_policy_handle_stage_count.argtypes = [C.c_void_p]
     lib.cn_policy_stage_ms.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     lib.cn_dsrnn_create.argtypes = [C.POINTER(CnDsrnnConfig), C.POINTER(C.c_void_p)]
     lib.cn_dsrnn_destroy.argtypes = [C.c_void_p]

@@ -11,6 +11,11 @@
 // human-human attention; spatial_linear = Linear(W, 128), ReLU, Linear(128, 256), ReLU runs straight on the compacted
 // spatial_edges rows (layer 1 in the embed1 slot, layer 2 into sout) and feeds the unchanged robot-human attention.
 //
+// visible_masks = 1 (the reference's sort_humans = False, selfAttn_srnn_temp_node.py:375-383, :398-416): the attention
+// masks are the caller's visible_masks instead of the detected_human_num prefix.  cn_mask_slots_kernel turns them into
+// per-environment counts and slot lists; the same scan then gives row_start / mc, and the two gathers (pack_inputs,
+// embed1) read slot row_slot[r] instead of r - row_start[e].  Every later kernel reads row_start / row_env only.
+//
 // gemm_mode 0: every layer on the fp32 CUDA-core GEMM (cn_gemm_f32_kernel).
 // gemm_mode 1: every layer with K >= 64 on the wgmma 3xFP16 GEMM (cn_gemm_tc_kernel): activations
 //              travel between layers as (hi, lo) fp16 pairs written by the producing kernel's epilogue.
@@ -33,7 +38,8 @@ struct cn_policy {
   cn_policy_config cfg;
   int N, H, Win, M;
   bool nsa;           // cfg.no_self_attn: spatial_linear(spatial_edges), no human-human attention
-  const char* const* stage_names;   // this network's stages (kStageNames or kStageNamesNsa)
+  bool vm;            // cfg.visible_masks: rows = the visible slots of cn_act_ptrs.visible_masks
+  const char* const* stage_names;   // this network's stages (kStageNames, kStageNamesNsa or their Vm variants)
   int num_stages;
   CnLaunchCtx lc;     // launch counter, PDL, first launch error, device allocations
   bool fuse_qkv;      // QKV projection + human-human attention in ONE kernel (cn_qkv_attn.cuh; opt-in, CN_FUSE_QKV=1)
@@ -70,6 +76,8 @@ struct cn_policy {
   std::vector<cudaEvent_t> ev;
   // workspace
   int *row_start, *row_env, *mc;
+  int *slot_tab, *row_slot;   // visible_masks only: [N * H] visible slots per environment, [M] slot of each row
+  float* vis_count;           // visible_masks only: [N] rows per environment (the scan's input)
   float *x16, *e1, *e2, *qkv, *ao, *sout, *xr, *rs, *t1, *u, *wv, *h0, *gi, *gh, *outb, *ac1, *a2, *c2;
   TcStoreMap qkv_st, sout_st;   // store maps of the fp32 outputs of the BN = 256 GEMMs (gemm_mode 1)
 };
@@ -117,6 +125,11 @@ const int kNumStages = sizeof(kStageNames) / sizeof(kStageNames[0]);
 const char* kStageNamesNsa[] = {"pack_inputs", "spatial_linear0", "spatial_linear2", "robot_branch_join",
                                 "hr_attention", "gru", "actor_critic_heads"};
 const int kNumStagesNsa = sizeof(kStageNamesNsa) / sizeof(kStageNamesNsa[0]);
+// visible_masks: the mask compaction first, then the stages above
+const char* kStageNamesVm[] = {"mask_rows", "pack_inputs", "embed1_gemm", "embed2_gemm", "qkv_gemm", "hh_attention",
+                               "outproj_spatial_gemm", "robot_branch_join", "hr_attention", "gru", "actor_critic_heads"};
+const char* kStageNamesNsaVm[] = {"mask_rows", "pack_inputs", "spatial_linear0", "spatial_linear2",
+                                  "robot_branch_join", "hr_attention", "gru", "actor_critic_heads"};
 
 inline void mark(cn_policy* p, cudaStream_t st, int i) {
   p->lc.cur_stage = i < p->num_stages ? p->stage_names[i] : "end";
@@ -131,7 +144,7 @@ int cn_policy_profile(cn_policy* p, int enable) {
   if (!p) return cn_set_error("cn_policy_profile: null argument");
   cudaSetDevice(p->cfg.device);
   if (enable && p->ev.empty()) {
-    p->ev.resize(kNumStages + 1);
+    p->ev.resize(p->num_stages + 1);
     for (auto& e : p->ev) cudaEventCreate(&e);
   }
   p->profile = enable != 0;
@@ -142,6 +155,7 @@ const char* cn_policy_stage_name(int i) { return (i >= 0 && i < kNumStages) ? kS
 const char* cn_policy_handle_stage_name(cn_policy* p, int i) {
   return (p && i >= 0 && i < p->num_stages) ? p->stage_names[i] : "";
 }
+int cn_policy_handle_stage_count(cn_policy* p) { return p ? p->num_stages : 0; }
 int cn_policy_stage_ms(cn_policy* p, float* out, int n) {
   if (!p || !out) return cn_set_error("cn_policy_stage_ms: null argument");
   if (p->ev.empty()) return cn_set_error("cn_policy_stage_ms: profiling was never enabled");
@@ -169,8 +183,9 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
   p->cfg = *cfg;
   p->N = cfg->num_envs; p->H = cfg->human_num; p->Win = cfg->input_size; p->M = p->N * p->H;
   p->nsa = cfg->no_self_attn != 0;
-  p->stage_names = p->nsa ? kStageNamesNsa : kStageNames;
-  p->num_stages = p->nsa ? kNumStagesNsa : kNumStages;
+  p->vm = cfg->visible_masks != 0;
+  p->stage_names = p->nsa ? (p->vm ? kStageNamesNsaVm : kStageNamesNsa) : (p->vm ? kStageNamesVm : kStageNames);
+  p->num_stages = (p->nsa ? kNumStagesNsa : kNumStages) + (p->vm ? 1 : 0);
   p->finalized = false; p->profile = false;
   cn_launch_init(&p->lc, cfg->device);
   {
@@ -208,6 +223,13 @@ int cn_policy_create(const cn_policy_config* cfg, cn_policy** out) {
     p->row_env = reinterpret_cast<int*>(q);
     if (!rc) rc = palloc(&p->lc, &q, 2 * N + 4);
     p->tile_tab = reinterpret_cast<int*>(q);
+    if (p->vm) {
+      if (!rc) rc = palloc(&p->lc, &q, M);
+      p->slot_tab = reinterpret_cast<int*>(q);
+      if (!rc) rc = palloc(&p->lc, &q, M + 1);
+      p->row_slot = reinterpret_cast<int*>(q);
+      if (!rc) rc = palloc(&p->lc, &p->vis_count, N);
+    }
   }
   WS(x16, M * 16); WS(e1, M * 128); WS(sout, M * 256);
   if (!p->nsa) { WS(e2, M * 512); WS(qkv, M * 1536); WS(ao, M * 512); }   // human-human attention only
@@ -440,19 +462,31 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   if (!d->robot_node || !d->temporal_edges || !d->spatial_edges || !d->detected_human_num || !d->h_in || !d->masks ||
       !d->value || !d->action || !d->log_prob || !d->h_out)
     return cn_set_error("cn_policy_act: missing input/output pointer");
+  if (p->vm && !d->visible_masks)
+    return cn_set_error("cn_policy_act: visible_masks is NULL, and this handle was created with visible_masks = 1 "
+                        "(sort_humans = False)");
   CnDeviceGuard guard(p->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
   const int N = p->N, H = p->H, M = p->M;
   const bool tcm = p->cfg.gemm_mode == 1;
   const int* mc = p->mc;
   const int ALL = 1 << 30;
-  mark(p, st, 0);
+  // o: stage index offset (visible_masks: stage 0 is the mask compaction)
+  const int o = p->vm ? 1 : 0;
+  if (p->vm) {
+    mark(p, st, 0);
+    launch_k(&p->lc, cn_mask_slots_kernel, dim3((N + 7) / 8), dim3(256), 0, st, d->visible_masks, N, H, p->vis_count,
+             p->slot_tab);
+  }
+  mark(p, st, o);
   // 0. compaction offsets, pack / pad inputs, h0 = h * mask
   {
-    launch_k(&p->lc, cn_row_offsets_kernel, dim3(1), dim3(1024), 0, st, d->detected_human_num, N, H, p->row_start, p->mc);
+    launch_k(&p->lc, cn_row_offsets_kernel, dim3(1), dim3(1024), 0, st, p->vm ? p->vis_count : d->detected_human_num, N, H,
+             p->row_start, p->mc);
     const int total = (!tcm && M * 16 > N * 128) ? M * 16 : N * 128;
-    launch_k(&p->lc, cn_pack_inputs_kernel, dim3((total + 255) / 256), dim3(256), 0, st, d->spatial_edges, p->Win, H, N, p->row_start, p->row_env,
-                                                               tcm ? nullptr : p->x16,
+    launch_k(&p->lc, p->vm ? cn_pack_inputs_kernel<true> : cn_pack_inputs_kernel<false>, dim3((total + 255) / 256), dim3(256), 0, st,
+                                                               d->spatial_edges, p->Win, H, N, p->row_start, p->row_env,
+                                                               p->slot_tab, p->row_slot, tcm ? nullptr : p->x16,
                                                                d->temporal_edges, d->robot_node, d->h_in, d->masks, p->xr,
                                                                p->h0, tcm ? p->tH0.hi : nullptr, tcm ? p->tH0.lo : nullptr);
   }
@@ -478,12 +512,12 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   }
   cudaEventRecord(p->ev_join, s2);
   // 1. human-human branch over the Mc = sum_e n_e valid rows (device-side count p->mc)
-  mark(p, st, 1);
+  mark(p, st, o + 1);
   if (tcm) {
-    launch_k(&p->lc, cn_embed1_kernel, dim3(p->lc.num_sms * 6), dim3(256), 0, st, d->spatial_edges, p->Win, H, p->row_start, p->row_env, p->mc, p->W1, p->b1,
-                                                     p->tE1.hi, p->tE1.lo);
+    launch_k(&p->lc, p->vm ? cn_embed1_kernel<true> : cn_embed1_kernel<false>, dim3(p->lc.num_sms * 6), dim3(256), 0, st,
+             d->spatial_edges, p->Win, H, p->row_start, p->row_env, p->row_slot, p->mc, p->W1, p->b1, p->tE1.hi, p->tE1.lo);
   } else gemm(p, st, p->x16, 16, p->W1, 16, p->b1, p->e1, 128, M, 128, 16, CN_ACT_RELU, 0, ALL, mc);
-  mark(p, st, 2);
+  mark(p, st, o + 2);
   if (p->nsa) {
     // no_self_attn: spatial_linear.2 + ReLU is the last per-human layer, straight into sout
     if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 256, 128, 256, p->b2, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
@@ -491,7 +525,7 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
   } else {
     if (tcm) gemm_tc(&p->lc, st, p->tE1, p->tW2, M, 512, 128, 256, p->b2, CN_ACT_RELU, out16(p->tE2), mc);
     else gemm(p, st, p->e1, 128, p->W2, 128, p->b2, p->e2, 512, M, 512, 128, CN_ACT_RELU, 0, ALL, mc);
-    mark(p, st, 3);
+    mark(p, st, o + 3);
     if (tcm) {
       // Optional experiment (CN_QKV_CHUNKS=2): QKV projection + attention in two row chunks split at an environment
       // boundary so that chunk 0's attention (side stream) overlaps chunk 1's GEMM.  Off by default: at H = 20 the
@@ -506,10 +540,10 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
         launch_k(&p->lc, cn_qkv_attn_kernel, dim3(p->lc.num_sms), dim3(QA_THREADS), QA_SMEM_BYTES, st, p->qa_ah, p->qa_al, p->qa_bh,
                  p->qa_bl, p->bqkvH, 1.0f / 64.0f, p->tile_tab, p->row_start, p->row_env, ah, al,
                  getenv("CN_QA_DBG") ? atoi(getenv("CN_QA_DBG")) : 0);
-        mark(p, st, 4);
+        mark(p, st, o + 4);
       } else if (p->qkv_chunks == 1) {
         gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc);
-        mark(p, st, 4);
+        mark(p, st, o + 4);
         launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, nullptr,
                                                                                nullptr, ah, al);
       } else {
@@ -520,18 +554,18 @@ int cn_policy_act(cn_policy* p, const cn_act_ptrs* d, void* stream) {
                                                                                 nullptr, ah, al);
       cudaEventRecord(p->ev_join3, p->st3);
       gemm_tc(&p->lc, st, p->tE2, p->tWqkv, M, 1536, 512, 256, p->bqkv, CN_ACT_NONE, out32(p->qkv, 1536, &p->qkv_st), mc, 0, 1 << 30, mid);
-      mark(p, st, 4);
+      mark(p, st, o + 4);
       launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, mc, mid, nullptr,
                                                                              ah, al);
       cudaStreamWaitEvent(st, p->ev_join3, 0);
       }
     } else {
       gemm(p, st, p->e2, 512, p->Wqkv, 512, p->bqkv, p->qkv, 1536, M, 1536, 512, CN_ACT_NONE, 0, ALL, mc);
-      mark(p, st, 4);
+      mark(p, st, o + 4);
       launch_k(&p->lc, p->attn_kernel, dim3(p->lc.num_sms * 64 / p->attn_warps), dim3(p->attn_warps * 32), 0, st, p->qkv, p->row_start, p->row_env, p->mc, nullptr,
                                                                              p->ao, nullptr, nullptr);
     }
-    mark(p, st, 5);
+    mark(p, st, o + 5);
     if (tcm) gemm_tc(&p->lc, st, p->tAo, p->tWos, M, 256, 512, 256, p->bos, CN_ACT_RELU, out32(p->sout, 256, &p->sout_st), mc);
     else gemm(p, st, p->ao, 512, p->Wos, 512, p->bos, p->sout, 256, M, 256, 512, CN_ACT_RELU, 0, ALL, mc);
   }
@@ -596,6 +630,7 @@ int64_t cn_policy_last_rows(cn_policy* p) {
 // so a test can read every stage's input and output back after cn_policy_act.  *kind = 0: fp32 at *ptr; 1: fp16
 // (hi, lo) pair at *ptr / *ptr_lo (value = hi + lo); 2: int32.  Row r of the buffer starts at element r * *ld.
 //   row_start [N + 1], row_env [Mc], mc [1]: compacted row layout (rows of environment e: row_start[e] .. [e + 1])
+//   row_slot [Mc] (visible_masks only): the slot of spatial_edges each compacted row holds
 //   e1 [Mc,128], e2 [Mc,512], qkv [Mc,1536] (not in the fused kernel's mode), ao [Mc,512], sout [Mc,256]
 //   rs [N,256], t1 [N,128], u [N,256], wv [N,256], h0 [N,128], gi / gh [N,384], h1 [N,128], ac1 [N,512],
 //   a2 / c2 [N,256];  folded weights Wqkv [1536,512], bqkv, Wos [256,512], bos, Woac [512,128], boac.
@@ -622,6 +657,10 @@ int cn_internal_policy_buffer(cn_policy* p, const char* name, void** ptr, void**
   if (s == "row_start") return i32(p->row_start, N + 1);
   if (s == "row_env") return i32(p->row_env, M);
   if (s == "mc") return i32(p->mc, 1);
+  if (s == "row_slot") {
+    if (!p->vm) return cn_set_error("cn_internal_policy_buffer: 'row_slot' exists with visible_masks = 1 only");
+    return i32(p->row_slot, M);
+  }
   if (p->nsa && (s == "e2" || s == "qkv" || s == "ao" || s == "Wqkv" || s == "bqkv" || s == "Wos" || s == "bos"))
     return cn_set_error("cn_internal_policy_buffer: '%s' does not exist without human-human attention (no_self_attn)", name);
   if (s == "e1") return tcm ? f16(p->tE1, M, 128) : f32(p->e1, M, 128, 128);

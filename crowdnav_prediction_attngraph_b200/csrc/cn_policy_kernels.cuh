@@ -209,10 +209,41 @@ __global__ void __launch_bounds__(1024) cn_row_offsets_kernel(const float* __res
   if (tid == 0) { *mc = carry; row_start[N] = carry; }
 }
 
-// Input packing: x16[row_start[e] + j, 16] = spatial_edges[e, j] zero-padded to K=16 for j < n_e;
-// xr[N,16] = cat(temporal_edges(2), robot_node(7)) zero padded; h0 = h_in * mask.
+// Row compaction by the visible mask (sort_humans = False, selfAttn_srnn_temp_node.py:375-383): the attention masks
+// are visible_masks, in slot (human id) order and not a prefix.  The argument above holds for any mask, so only the
+// choice of rows changes.  One warp per environment: slot_tab[e * H + k] = the k-th visible slot in ascending order
+// (ballot + popc of the lower lanes per 32 slots) and count[e] = the number of visible slots, as a float so that
+// cn_row_offsets_kernel scans it as it scans detected_human_num.  An environment with no visible human keeps slot 0
+// only (the reference's dummy_human_mask, :351-358, :382-383).
+__global__ void __launch_bounds__(256) cn_mask_slots_kernel(const uint8_t* vis /* [N, H], nonzero = visible */, int N,
+                                                            int H, float* __restrict__ count, int* __restrict__ slot_tab) {
+  cn_pdl_prologue();
+  const int lane = threadIdx.x & 31;
+  const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (e >= N) return;
+  const uint8_t* m = vis + (size_t)e * H;
+  int* tab = slot_tab + (size_t)e * H;
+  int n = 0;
+  for (int s0 = 0; s0 < H; s0 += 32) {
+    const int s = s0 + lane;
+    const bool v = s < H && m[s] != 0;
+    const unsigned b = __ballot_sync(0xffffffffu, v);
+    if (v) tab[n + __popc(b & ((1u << lane) - 1u))] = s;
+    n += __popc(b);
+  }
+  if (lane == 0) {
+    if (n == 0) { tab[0] = 0; n = 1; }
+    count[e] = (float)n;
+  }
+}
+
+// Input packing: x16[row_start[e] + j, 16] = spatial_edges[e, s] zero-padded to K=16 for j < n_e, with s = j
+// (kSlot false: the first n_e rows, sorted humans) or s = slot_tab[e * H + j] (kSlot true: the visible slots, and
+// row_slot[row_start[e] + j] = s); xr[N,16] = cat(temporal_edges(2), robot_node(7)) zero padded; h0 = h_in * mask.
+template <bool kSlot>
 __global__ void cn_pack_inputs_kernel(const float* __restrict__ spatial, int Win, int H, int N,
                                       const int* __restrict__ row_start, int* __restrict__ row_env,
+                                      const int* __restrict__ slot_tab, int* __restrict__ row_slot,
                                       float* __restrict__ x16,
                                       const float* __restrict__ temporal, const float* __restrict__ robot,
                                       const float* __restrict__ h_in, const float* __restrict__ masks,
@@ -225,13 +256,20 @@ __global__ void cn_pack_inputs_kernel(const float* __restrict__ spatial, int Win
     const int e = r / H, j = r - e * H;
     const int rs = row_start[e], n = row_start[e + 1] - rs;
     if (j < n) {
-      x16[(size_t)(rs + j) * 16 + c] = c < Win ? spatial[(size_t)r * Win + c] : 0.0f;
-      if (c == 0) row_env[rs + j] = e;
+      const int s = kSlot ? slot_tab[r] : j;
+      x16[(size_t)(rs + j) * 16 + c] = c < Win ? spatial[((size_t)e * H + s) * Win + c] : 0.0f;
+      if (c == 0) {
+        row_env[rs + j] = e;
+        if (kSlot) row_slot[rs + j] = s;
+      }
     }
   }
-  if (!x16 && idx < N) {                  // tensor-core mode: row -> environment map of the compacted rows
+  if (!x16 && idx < N) {                  // tensor-core mode: row -> environment (and slot) map of the compacted rows
     const int rs = row_start[idx], n = row_start[idx + 1] - rs;
-    for (int j = 0; j < n; ++j) row_env[rs + j] = idx;
+    for (int j = 0; j < n; ++j) {
+      row_env[rs + j] = idx;
+      if (kSlot) row_slot[rs + j] = slot_tab[(size_t)idx * H + j];
+    }
   }
   if (idx < N * 16) {
     const int e = idx >> 4, c = idx & 15;
@@ -259,8 +297,11 @@ __global__ void cn_pack_inputs_kernel(const float* __restrict__ spatial, int Win
 // tensor-core tile: one warp per compacted human row, lane l owns outputs 4l..4l+3, the 128 x 16 weights sit
 // transposed in shared memory (conflict-free LDS.128), the input row is broadcast by shuffles, and each lane
 // issues one 8-byte store per half (256 B coalesced per warp).  Latency bound: sized for many resident warps.
+// kSlot: row r gathers slot row_slot[r] (visible-mask compaction) instead of slot r - row_start[e].
+template <bool kSlot>
 __global__ void __launch_bounds__(256) cn_embed1_kernel(const float* __restrict__ spatial, int Win, int H,
                                                         const int* __restrict__ row_start, const int* __restrict__ row_env,
+                                                        const int* __restrict__ row_slot,
                                                         const int* __restrict__ mc_ptr,
                                                         const float* __restrict__ W1 /* [128][16], zero padded */,
                                                         const float* __restrict__ b1, __half* __restrict__ e_hi,
@@ -275,7 +316,7 @@ __global__ void __launch_bounds__(256) cn_embed1_kernel(const float* __restrict_
   const int mc = *mc_ptr;
   for (int r = gw; r < mc; r += nw) {
     const int e = row_env[r];
-    const int j = r - row_start[e];
+    const int j = kSlot ? row_slot[r] : r - row_start[e];
     const float x = lane < Win ? __ldg(spatial + ((size_t)e * H + j) * Win + lane) : 0.0f;
     float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
 #pragma unroll

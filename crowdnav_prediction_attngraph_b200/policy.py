@@ -95,14 +95,17 @@ def make_reference_like_state_dict(input_size=12, seed=0, self_attn=True):
 
 class CudaPolicy(object):
     """Thin handle on cn_policy: upload a reference state_dict, run the rollout forward.  self_attn=False runs the
-    reference's use_self_attn = False network (cn_policy_config.no_self_attn)."""
+    reference's use_self_attn = False network (cn_policy_config.no_self_attn).  visible_masks=True is the reference's
+    sort_humans = False: act() masks the attention with obs['visible_masks'] (cn_policy_config.visible_masks)."""
 
-    def __init__(self, num_envs, human_num, input_size=12, device="cuda:0", gemm_mode=1, self_attn=True):
+    def __init__(self, num_envs, human_num, input_size=12, device="cuda:0", gemm_mode=1, self_attn=True,
+                 visible_masks=False):
         self._setup(num_envs, human_num, input_size, device)
         self.self_attn = bool(self_attn)
+        self.visible_masks = bool(visible_masks)
         cfg = _capi.CnPolicyConfig(num_envs, human_num, input_size,
                                    self.device.index if self.device.index is not None else 0, gemm_mode,
-                                   0 if self.self_attn else 1)
+                                   0 if self.self_attn else 1, 1 if self.visible_masks else 0)
         self._h = C.c_void_p()
         _capi.check(self.lib, self.lib.cn_policy_create(C.byref(cfg), C.byref(self._h)), "cn_policy_create")
 
@@ -186,11 +189,18 @@ class CudaPolicy(object):
         args = self._inputs(robot_node=obs["robot_node"], temporal_edges=obs["temporal_edges"],
                             spatial_edges=obs["spatial_edges"], detected_human_num=obs["detected_human_num"],
                             h_in=h, masks=masks)
+        vm = None
+        if self.visible_masks:
+            vm = obs["visible_masks"]           # one byte per slot, as the environment writes it
+            if vm.dtype not in (torch.bool, torch.uint8) or not vm.is_contiguous() or vm.device != self.device:
+                vm = vm.to(self.device, torch.bool).contiguous()
+            args["visible_masks"] = vm
         ptrs = _capi.CnActPtrs(
             args["robot_node"].data_ptr(), args["temporal_edges"].data_ptr(), args["spatial_edges"].data_ptr(),
             args["detected_human_num"].data_ptr(), args["h_in"].data_ptr(), args["masks"].data_ptr(),
             None if deterministic else noise.data_ptr(), b["value"].data_ptr(), b["action"].data_ptr(),
-            b["log_prob"].data_ptr(), b["h_out"].data_ptr(), b["mean"].data_ptr())
+            b["log_prob"].data_ptr(), b["h_out"].data_ptr(), b["mean"].data_ptr(),
+            None if vm is None else vm.data_ptr())
         rc = self.lib.cn_policy_act(self._h, C.byref(ptrs), self._stream())     # restores the caller's device itself
         if rc:
             _capi.check(self.lib, rc, "cn_policy_act")
@@ -208,7 +218,7 @@ class CudaPolicy(object):
     def stage_ms(self):
         """{stage: ms} of the last act, under this handle's own stage names (profiling must have been enabled with
         profile(True) before it)."""
-        n = self.lib.cn_policy_stage_count()
+        n = self.lib.cn_policy_handle_stage_count(self._h)
         out = (C.c_float * n)()
         _capi.check(self.lib, self.lib.cn_policy_stage_ms(self._h, out, n), "cn_policy_stage_ms")
         names = [self.lib.cn_policy_handle_stage_name(self._h, i).decode() for i in range(n)]
@@ -395,7 +405,9 @@ class Policy(nn.Module):
     """Drop-in for rl.networks.model.Policy(obs_space.spaces, action_space, base_kwargs=args, base=...).
 
     args.use_self_attn = False (selfAttn_merge_srnn only; True when absent) is the reference's ablation without
-    human-human attention.  args.use_hr_attn is accepted and changes nothing: the reference never reads it."""
+    human-human attention.  args.sort_humans = False (selfAttn_merge_srnn only; True when absent) masks both
+    attentions with inputs['visible_masks'] instead of the detected_human_num prefix (selfAttn_srnn_temp_node.py:
+    375-383).  args.use_hr_attn is accepted and changes nothing: the reference never reads it."""
 
     def __init__(self, obs_shape, action_space, base=None, base_kwargs=None):
         super().__init__()
@@ -412,6 +424,8 @@ class Policy(nn.Module):
         check_widths(args, 'srnn' if self.dsrnn else 'selfAttn_merge_srnn')
         # the reference's SRNN ignores use_self_attn (srnn_model.py); older argument files lack it (True)
         self.self_attn = self.dsrnn or bool(getattr(args, 'use_self_attn', True))
+        # the SRNN never reads sort_humans either; older argument files lack it (True, :376-377)
+        self.sort_humans = self.dsrnn or bool(getattr(args, 'sort_humans', True))
         sp = obs_shape['spatial_edges'].shape
         self.human_num, self.input_size = int(sp[0]), int(sp[1])
         self.nenv = int(getattr(args, 'num_processes', 1)) if args is not None else 1
@@ -444,7 +458,8 @@ class Policy(nn.Module):
                 self._cuda = CudaDsrnn(N, self.human_num, self.input_size, device=device)
             else:
                 self._cuda = CudaPolicy(N, self.human_num, self.input_size, device=device,
-                                        gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")), self_attn=self.self_attn)
+                                        gemm_mode=int(os.environ.get("CN_GEMM_MODE", "1")), self_attn=self.self_attn,
+                                        visible_masks=not self.sort_humans)
             self._cuda_version = -1
         # parameter objects are fixed after construction: walk the module tree once, then only read the
         # version counters (the tree walk alone cost ~0.1 ms of host time per act)
@@ -492,8 +507,14 @@ class Policy(nn.Module):
         H = self.human_num
         dt = b.robot_linear[0].weight.dtype            # fp32; fp64 when a test runs the module in double as its reference
         sp = inputs['spatial_edges'].reshape(T * N, H, -1).to(dt)
-        n = inputs['detected_human_num'].reshape(T * N).long().clamp(1, H)
-        valid = torch.arange(H, device=sp.device)[None, :] < n[:, None]
+        if self.sort_humans:
+            n = inputs['detected_human_num'].reshape(T * N).long().clamp(1, H)
+            valid = torch.arange(H, device=sp.device)[None, :] < n[:, None]
+        else:
+            # visible_masks, and slot 0 alone for a sample that sees nobody (dummy_human_mask, :351-358, :382-383)
+            valid = inputs['visible_masks'].reshape(T * N, H).bool().clone()
+            valid[:, 0] |= ~valid.any(1)
+            n = valid.sum(1)
         rs = b.robot_linear(torch.cat([inputs['temporal_edges'].reshape(T * N, 2),
                                        inputs['robot_node'].reshape(T * N, 7)], -1).to(dt))
         B = T * N

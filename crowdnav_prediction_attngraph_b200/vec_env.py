@@ -112,7 +112,9 @@ def _check_collect(config, seed, phase, nenv_total):
 def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None, rank_offset=0, device_index=0,
                                phase=None, allow_unsorted=False):
     """Snapshot a reference `Config` object (crowd_nav/configs/config.py) into the flat cn_config.
-    phase None follows rl/networks/envs.py:55-58: one environment -> 'test', more -> 'train'."""
+    phase None follows rl/networks/envs.py:55-58: one environment -> 'test', more -> 'train'.
+    args.sort_humans = False is taken on every environment but CrowdSimPred-v0; `allow_unsorted` is accepted and
+    changes nothing (it once opened sort_humans = False behind the GST wrapper only)."""
     if phase is None:
         phase = "test" if (nenv_total or num_envs) == 1 else "train"
     if phase not in ("train", "test"):
@@ -154,12 +156,14 @@ def config_dict_from_reference(config, num_envs, seed, env_name, nenv_total=None
                                       "simulator would be rebuilt as humans join and leave)" % (config.robot.policy,))
     if env_name == COLLECT_ENV:
         seed = _check_collect(config, seed, phase, nenv_total or num_envs)
-        allow_unsorted = True           # the collect observation is never sorted
     sort_humans = getattr(getattr(config, "args", None), "sort_humans", True)
-    if not sort_humans and not allow_unsorted:
-        # the policy mirror masks attention with detected_human_num, which is only valid for distance-sorted rows
-        # (selfAttn_srnn_temp_node.py:398-404 uses visible_masks otherwise); the GST wrapper sorts on its own
-        raise NotImplementedError("args.sort_humans=False is covered only behind the GST wrapper (pretext_wrapper=True)")
+    if not sort_humans and env_name == "CrowdSimPred-v0":
+        # with sort_humans = False the policy masks its attention with obs['visible_masks']
+        # (selfAttn_srnn_temp_node.py:378-383), and CrowdSimPred-v0's observation has no such key
+        raise NotImplementedError(
+            "args.sort_humans=False on CrowdSimPred-v0 is not covered: the reference cannot run it (its policy reads "
+            "inputs['visible_masks'], which CrowdSimPred-v0's observation does not have, crowd_sim_pred.py:45-55, "
+            "and raises KeyError)")
     return _capi.default_config_dict(
         num_envs=num_envs, nenv_total=nenv_total or num_envs, rank_offset=rank_offset, seed=seed,
         human_num=config.sim.human_num, human_num_range=int(config.sim.human_num_range),

@@ -228,6 +228,12 @@ typedef struct cn_policy_config {
                         /* base.spatial_linear.0 [128, input_size] and .2 [256, 128] (+ biases)  */
                         /* and no base.spatial_attn.* key; CN_FUSE_QKV / CN_ATTN_R /             */
                         /* CN_QKV_CHUNKS have no effect.  A zeroed field keeps today's network.  */
+  int32_t visible_masks; /* 0: the attention masks are the detected_human_num prefix (sorted      */
+                        /* humans, the reference's sort_humans = True).  1: sort_humans = False:  */
+                        /* the masks are cn_act_ptrs.visible_masks, in slot order, and an env    */
+                        /* with no visible human keeps slot 0 only (dummy_human_mask);           */
+                        /* detected_human_num is not read.  Either network.  A zeroed field     */
+                        /* keeps the prefix.                                                     */
 } cn_policy_config;
 
 int cn_policy_create(const cn_policy_config *cfg, cn_policy **out);
@@ -251,12 +257,15 @@ typedef struct cn_act_ptrs {
   float *log_prob;      /* [N,1]                                                                */
   float *h_out;         /* [N,1,128]                                                            */
   float *action_mean;   /* [N,2] (dist.fc_mean output; parity tests)                            */
+  /* input, required by a handle created with visible_masks = 1 and ignored otherwise           */
+  const uint8_t *visible_masks; /* [N,H] one byte per slot, nonzero = visible (a torch.bool tensor) */
 } cn_act_ptrs;
 
 /* replaces: Policy.act (rl/networks/model.py:56-74) with infer=True.                           */
 int cn_policy_act(cn_policy *pol, const cn_act_ptrs *d, void *stream);
 int64_t cn_policy_launch_count(cn_policy *pol);
-/* Rows (valid humans, sum over envs of detected_human_num) the last cn_policy_act processed;
+/* Rows (valid humans, sum over envs of detected_human_num, or of the visible slots with a
+ * visible_masks handle) the last cn_policy_act processed;
  * synchronises the device.  The per-human pipeline runs on these compacted rows only.          */
 int64_t cn_policy_last_rows(cn_policy *pol);
 
@@ -266,11 +275,14 @@ int64_t cn_policy_last_rows(cn_policy *pol);
  * Stage names: cn_policy_stage_name(i), i < cn_policy_stage_count().                            *
  * A no_self_attn handle has fewer stages (spatial_linear0, spatial_linear2 in place of the five *
  * human-human stages): cn_policy_handle_stage_name(pol, i) names the handle's own stage i and   *
- * returns "" past its last one; cn_policy_stage_count() bounds every handle's count.            */
+ * returns "" past its last one.  A visible_masks handle has one more stage, mask_rows (the     *
+ * visible-mask row compaction), before pack_inputs.  cn_policy_handle_stage_count(pol) is the   *
+ * handle's own count.                                                                          */
 int cn_policy_profile(cn_policy *pol, int enable);
 int cn_policy_stage_count(void);
 const char *cn_policy_stage_name(int i);
 const char *cn_policy_handle_stage_name(cn_policy *pol, int i);
+int cn_policy_handle_stage_count(cn_policy *pol);
 int cn_policy_stage_ms(cn_policy *pol, float *out, int n);
 
 /* ------------------------------------------------------------------------------------------ */

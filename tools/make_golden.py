@@ -139,6 +139,14 @@ CASES = {
     "env_pred_h8_sf_truth_test_rand": dict(env_name="CrowdSimPred-v0", human_num=8, predict_method="truth",
                                            human_policy="social_force", randomize=True, goal_changing=True, nenv=2,
                                            steps=160, seed=21, phase="test"),
+    # args.sort_humans = False on CrowdSimVarNum-v0: row humans[i].id holds human i and visible_masks[:human_num] is
+    # set by position (crowd_sim_var_num.py:258-268); with human_num_range > 0 the two can disagree
+    "env_varnum_h20_unsorted_rand": dict(env_name="CrowdSimVarNum-v0", human_num=20, predict_method="none",
+                                         sort_humans=False, randomize=True, goal_changing=True, nenv=2, steps=160,
+                                         seed=31),
+    "env_varnum_h6_range2_unsorted": dict(env_name="CrowdSimVarNum-v0", human_num=6, predict_method="none",
+                                          human_num_range=2, sort_humans=False, randomize=True, goal_changing=True,
+                                          nenv=2, steps=200, seed=13),
 }
 
 
@@ -173,6 +181,7 @@ def build_reference_env(case, rank):
     cfg.humans.random_goal_changing = case["goal_changing"]
     cfg.orca.neighbor_dist = 10
     cfg.robot.visible = case.get("robot_visible", False)
+    cfg.args.sort_humans = case.get("sort_humans", True)
     if "human_fov" in case:
         cfg.humans.FOV = case["human_fov"]
     env = gym.make(case["env_name"])

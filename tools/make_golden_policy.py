@@ -15,7 +15,10 @@ env_varnum_h20_vis_rand).  Weights: tests/policy_no_self_attn_ref.synth_state_di
 shared with the full network; spatial_linear.0 / .2 from the reference's orthogonal initialiser with seeded
 generators).  Each file also holds the reference module's state_dict keys and shapes.
 
-    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_policy.py [--no-self-attn]
+--unsorted writes the fixtures of args.sort_humans = False (unsorted_fixtures below): policy_unsorted_{full,nsa}_
+{varnum,h20,h50}.
+
+    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_policy.py [--no-self-attn | --unsorted]
 """
 import os
 import sys
@@ -125,10 +128,56 @@ def no_self_attn_fixtures():
                             sd_keys=np.array(keys), sd_shapes=np.array([str(tuple(sd[k].shape)) for k in keys]))
 
 
+def unsorted_fixtures():
+    """args.sort_humans = False: both attentions masked with inputs['visible_masks'] (selfAttn_srnn_temp_node.py:375-383)
+    instead of the detected_human_num prefix, for the full network (synthetic fill) and the use_self_attn = False
+    ablation.  W = 2: 64 observations of the env_varnum_h20_unsorted_rand rollout (CrowdSimVarNum-v0 with sort_humans =
+    False), eight of them with every mask cleared (the reference's dummy_human_mask).  W = 12: the GST wrapper's outputs
+    (rows sorted by distance, masks in id order) of gst_rollout (H = 20) and gst_rollout_h50."""
+    sys.path.insert(0, os.path.join(REPO, "tests"))
+    from tests.policy_fixture import synth_state_dict
+    from tests.policy_no_self_attn_ref import synth_state_dict_nsa
+    keys = ["robot_node", "temporal_edges", "spatial_edges", "detected_human_num", "visible_masks"]
+    for src, prefix, H, W in [("env_varnum_h20_unsorted_rand", "ob_", 20, 2), ("gst_rollout", "fin_", 20, 12),
+                              ("gst_rollout_h50", "fin_", 50, 12)]:
+        g = np.load(os.path.join(REPO, "tests", "golden", src + ".npz"))
+        T1, N = g[prefix + "robot_node"].shape[:2]
+        B = 64
+        idx = np.random.RandomState(0).choice(T1 * N, B, replace=False)
+        obs = {k: torch.from_numpy(g[prefix + k].reshape(T1 * N, *g[prefix + k].shape[2:])[idx]) for k in keys}
+        obs = {k: v if k == "visible_masks" else v.float() for k, v in obs.items()}
+        if W == 2:
+            obs["visible_masks"][::8] = False
+        gen = torch.Generator().manual_seed(123)
+        h = torch.randn(B, 1, 128, generator=gen) * 0.5
+        masks = (torch.rand(B, 1, generator=gen) > 0.1).float()
+        env_name = "CrowdSimVarNum-v0" if W == 2 else "CrowdSimPred-v0"
+        for net, use_sa in [("full", True), ("nsa", False)]:
+            pol = build_reference_policy(env_name, H, W, B, use_self_attn=use_sa)
+            pol.base.args.sort_humans = False
+            sd = pol.state_dict()
+            pol.load_state_dict(synth_state_dict(sd) if use_sa else synth_state_dict_nsa(sd))
+            rnn = {"human_node_rnn": h.clone(), "human_human_edge_rnn": torch.zeros(B, H + 1, 256)}
+            with torch.no_grad():
+                value, feat, hx = pol.base({k: v.clone() for k, v in obs.items()}, rnn, masks.clone(), infer=True)
+                mean = pol.dist.fc_mean(feat)
+            name = "policy_unsorted_%s_%s" % (net, "varnum" if W == 2 else "h%d" % H)
+            vis = obs["visible_masks"].numpy()
+            print(name, "value range", float(value.min()), float(value.max()), "visible", float(vis.sum(1).mean()),
+                  "none visible", int((vis.sum(1) == 0).sum()),
+                  "non-prefix", int(sum(not vis[i, :vis[i].sum()].all() for i in range(B))))
+            np.savez_compressed(os.path.join(REPO, "tests", "golden", name + ".npz"),
+                                h=h.numpy(), masks=masks.numpy(), **{"ob_" + k: v.numpy() for k, v in obs.items()},
+                                synth_value=value.numpy(), synth_mean=mean.numpy(), synth_h=hx["human_node_rnn"].numpy())
+
+
 def long_h20_recording():
     """The 260-step env_pred_h20 rollout of the reference (the committed fixture keeps only its first steps)."""
     import make_golden
     return make_golden.run_case("env_pred_h20", dict(make_golden.CASES["env_pred_h20"], steps=make_golden.LONG_H20_STEPS))
 
 if __name__ == "__main__":
-    no_self_attn_fixtures() if "--no-self-attn" in sys.argv[1:] else main()
+    if "--unsorted" in sys.argv[1:]:
+        unsorted_fixtures()
+    else:
+        no_self_attn_fixtures() if "--no-self-attn" in sys.argv[1:] else main()

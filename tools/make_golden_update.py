@@ -17,7 +17,12 @@ fit a fixture), compared entry by entry by tests/test_update_parity_reference.py
 (args.use_self_attn = False; weights tests/policy_no_self_attn_ref.synth_state_dict_nsa):
 update_nsa_t30_n8.npz and update_nsa_t30_n8_entries.npz.
 
-    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_update.py [--no-self-attn]
+--unsorted records the same two files for args.sort_humans = False (both attentions masked with visible_masks), on a
+rollout of CrowdSimVarNum-v0 with unsorted observations (W = 2): four 30-step windows of each of the two environments
+of tests/golden/env_varnum_h20_unsorted_rand.npz, every observation key, visible_masks included, through the reference
+storage.  Weights: the full network's synthetic fill.  update_unsorted_t30_n8.npz and update_unsorted_t30_n8_entries.npz.
+
+    CROWDNAV_REFERENCE_ROOT=<reference checkout> python tools/make_golden_update.py [--no-self-attn | --unsorted]
 """
 import os
 import sys
@@ -37,6 +42,10 @@ HYPER = dict(clip_param=0.2, ppo_epoch=2, num_mini_batch=2, value_loss_coef=0.5,
              lr=4e-5, eps=1e-5, max_grad_norm=0.5)
 SEED_GEN = 777
 USE_SELF_ATTN = "--no-self-attn" not in sys.argv[1:]
+UNSORTED = "--unsorted" in sys.argv[1:]
+if UNSORTED:
+    W = 2
+OBS_KEYS = ["robot_node", "temporal_edges", "spatial_edges", "detected_human_num"] + (["visible_masks"] if UNSORTED else [])
 
 
 def synth(template):
@@ -47,8 +56,8 @@ def synth(template):
     return synth_state_dict_nsa(template)
 
 
-def pick_windows(done):
-    """two window starts per source env such that every window holds at least one episode end in steps 3..26"""
+def pick_windows(done, per_env=2):
+    """`per_env` window starts per source env such that every window holds at least one episode end in steps 3..26"""
     starts = []
     for e in range(done.shape[1]):
         idx = np.nonzero(done[:, e])[0]
@@ -57,18 +66,19 @@ def pick_windows(done):
             s = int(d) - 11
             if s >= 0 and s + T < done.shape[0] and all(abs(s - g) >= 8 for g in got):
                 got.append(s)
-            if len(got) == 2:
+            if len(got) == per_env:
                 break
-        assert len(got) == 2, (e, idx)
+        assert len(got) == per_env, (e, idx)
         starts.append(got)
     return starts
 
 
 def cut_rollout(g):
-    starts = pick_windows(g["done"])
-    cols = [(e, s) for e in range(4) for s in starts[e]]          # 8 (source env, start) pairs
+    ne = g["done"].shape[1]                                       # 4 source envs (env_pred_h20) or 2 (unsorted VarNum)
+    starts = pick_windows(g["done"], N // ne)
+    cols = [(e, s) for e in range(ne) for s in starts[e]]         # 8 (source env, start) pairs
     ob = {}
-    for k in ["robot_node", "temporal_edges", "spatial_edges", "detected_human_num"]:
+    for k in OBS_KEYS:
         ob[k] = np.stack([g["ob_" + k][s:s + T + 1, e] for e, s in cols], 1).astype(np.float32)
     act = np.stack([g["actions"][s:s + T, e] for e, s in cols], 1).astype(np.float32)
     rew = np.stack([g["reward"][s:s + T, e] for e, s in cols], 1).astype(np.float32)
@@ -79,8 +89,11 @@ def cut_rollout(g):
 def reference_objects():
     from make_golden_policy import build_reference_policy
     argv = sys.argv
-    pol = build_reference_policy("CrowdSimPred-v0", H, W, N, use_self_attn=USE_SELF_ATTN)
+    pol = build_reference_policy("CrowdSimVarNum-v0" if UNSORTED else "CrowdSimPred-v0", H, W, N,
+                                 use_self_attn=USE_SELF_ATTN)
     sys.argv = argv
+    if UNSORTED:
+        pol.base.args.sort_humans = False
     pol.base.nminibatch = HYPER["num_mini_batch"]
     pol.base.seq_length = T
     pol.load_state_dict(synth(pol.state_dict()))
@@ -115,6 +128,8 @@ def spaces_for_reference():
     import gym
     sp = {"robot_node": gym.spaces.Box(-np.inf, np.inf, (1, 7)), "temporal_edges": gym.spaces.Box(-np.inf, np.inf, (1, 2)),
           "spatial_edges": gym.spaces.Box(-np.inf, np.inf, (H, W)), "detected_human_num": gym.spaces.Box(-np.inf, np.inf, (1,))}
+    if UNSORTED:
+        sp["visible_masks"] = gym.spaces.Box(-np.inf, np.inf, (H,))
     return sp, gym.spaces.Box(-np.inf * np.ones(2), np.inf * np.ones(2), dtype=np.float32)
 
 
@@ -123,7 +138,9 @@ def run_reference():
     from rl.networks.storage import RolloutStorage
     from rl.ppo import PPO
     from make_golden_policy import long_h20_recording
-    ob, act, rew, done = cut_rollout(long_h20_recording())
+    src = np.load(os.path.join(REPO, "tests", "golden", "env_varnum_h20_unsorted_rand.npz")) if UNSORTED \
+        else long_h20_recording()
+    ob, act, rew, done = cut_rollout(src)
     pol = reference_objects()
     spaces, act_space = spaces_for_reference()
     ro = fill_storage(pol, RolloutStorage, ob, act, rew, done, spaces, act_space)
@@ -183,7 +200,7 @@ def sample_entries(pol):
 
 if __name__ == "__main__":
     out, ref_pol = run_reference()
-    tag = "update_t30_n8" if USE_SELF_ATTN else "update_nsa_t30_n8"
+    tag = "update_unsorted_t30_n8" if UNSORTED else ("update_t30_n8" if USE_SELF_ATTN else "update_nsa_t30_n8")
     p = os.path.join(REPO, "tests", "golden", tag + ".npz")
     np.savez_compressed(p, **out)
     np.savez_compressed(os.path.join(REPO, "tests", "golden", tag + "_entries.npz"), **sample_entries(ref_pol))
