@@ -460,4 +460,46 @@ int cn_dsrnn_stage_ms(cn_dsrnn* p, float* out, int n) {
 
 int64_t cn_dsrnn_launch_count(cn_dsrnn* p) { return p ? p->lc.launches : 0; }
 
+// Internal test hook (not part of the public header): where a workspace buffer of the forward lives, so a test can read
+// every stage's input and output back after cn_dsrnn_act.  *kind = 0: fp32 at *ptr; 1: fp16 (hi, lo) pair at *ptr /
+// *ptr_lo (value = hi + lo); 2: int32 (none here).  Row r of the buffer starts at element r * *ld.
+//   As [N H, 320], At [N, 320]  split A operands of the spatial / temporal edge GRUs: [x_emb | m h]
+//   HW [N, 512]                 split [h_t' | wv] (h_t' from the temporal GRU's epilogue, wv from the attention)
+//   te [N, 64], Te [N, 64]      temporal_edge_layer(h_t'), fp32 and split
+//   u, wv [N, 256]              W_s^T te and the attention's fp32 output
+//   T1 [N, 128]                 split node-GRU input [enc | emb]
+//   h0 [N, 128], H0 [N, 128]    h_in * mask, fp32 and split
+//   gi, gh [N, 384]             node-GRU pre-activations
+//   H1 [N, 128]                 split h_out
+//   Ac1 [N, 512], a2, c2 [N, 256]  tanh([actor.0 | critic.0] o output_linear), actor.2, critic.2
+int cn_internal_dsrnn_buffer(cn_dsrnn* p, const char* name, void** ptr, void** ptr_lo, int* rows, int* cols, int* ld,
+                             int* kind) {
+  if (!p || !name || !ptr || !ptr_lo || !rows || !cols || !ld || !kind)
+    return cn_set_error("cn_internal_dsrnn_buffer: null argument");
+  const int N = p->N;
+  const std::string s(name);
+  *ptr_lo = nullptr;
+  auto f32 = [&](const float* q, int r, int c) { *ptr = (void*)q; *rows = r; *cols = c; *ld = c; *kind = 0; return 0; };
+  auto f16 = [&](const TcMat& t, int r, int c) {
+    *ptr = t.hi; *ptr_lo = t.lo; *rows = r; *cols = c; *ld = t.pitch; *kind = 1; return 0;
+  };
+  if (s == "As") return f16(p->tAs, N * p->H, kK);
+  if (s == "At") return f16(p->tAt, N, kK);
+  if (s == "HW") return f16(p->tHW, N, 512);
+  if (s == "te") return f32(p->te, N, 64);
+  if (s == "Te") return f16(p->tTe, N, 64);
+  if (s == "u") return f32(p->u, N, 256);
+  if (s == "wv") return f32(p->wv, N, 256);
+  if (s == "T1") return f16(p->tT1, N, 128);
+  if (s == "h0") return f32(p->h0, N, 128);
+  if (s == "H0") return f16(p->tH0, N, 128);
+  if (s == "gi") return f32(p->gi, N, 384);
+  if (s == "gh") return f32(p->gh, N, 384);
+  if (s == "H1") return f16(p->tH1, N, 128);
+  if (s == "Ac1") return f16(p->tAc1, N, 512);
+  if (s == "a2") return f32(p->a2, N, 256);
+  if (s == "c2") return f32(p->c2, N, 256);
+  return cn_set_error("cn_internal_dsrnn_buffer: unknown buffer '%s'", name);
+}
+
 }  // extern "C"

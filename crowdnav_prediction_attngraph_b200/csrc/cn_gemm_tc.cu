@@ -308,6 +308,34 @@ int cn_internal_gemm_tc(const float* dA, const float* dW, const float* dbias, fl
                         int bn) {
   return cn_internal_gemm_tc_ex(dA, dW, dbias, dC, M, N, K, act, bn, nullptr, nullptr, 0, 0, nullptr, nullptr, 0, 0, 0);
 }
+// The edge-GRU instance (TC_OUT_GRU, gemm_tc_gru) on its own: A fp32 [M, 320] = [x | m h] split at scale 1, dB fp32
+// [1024, 320] and dbias [1024] already interleaved (cn_dsrnn.cu, interleave_gru) and split at scale 64, as in the
+// rollout.  h_in (null: zero state), mask and h_out are indexed as gemm_tc_gru documents (h_out needs
+// ceil(M / group) * pitch rows of 256); out_hi / out_lo (both or neither): split copy of h' [M, ldh].
+int cn_internal_gemm_tc_gru(const float* dA, const float* dB, const float* dbias, const float* h_in, const float* mask,
+                            float* h_out, int M, int group, int pitch, int off, __half* out_hi, __half* out_lo, int ldh) {
+  const int N = 4 * 256, K = 64 + 256;
+  if (M <= 0 || group <= 0 || off < 0 || off + group > pitch || !dA || !dB || !dbias || !mask || !h_out ||
+      (!out_hi != !out_lo) || (out_hi && (ldh < 256 || ldh % 2)))
+    return cn_set_error("cn_internal_gemm_tc_gru: need M, group > 0, 0 <= off, off + group <= pitch, A, B, bias, mask "
+                        "and h_out, and out_hi / out_lo both or neither with an even ldh >= 256");
+  CnLaunchCtx ctx;                                 // no PDL
+  cudaDeviceGetAttribute(&ctx.num_sms, cudaDevAttrMultiProcessorCount, 0);
+  TcMat A, B;
+  int rc = tc_alloc(&ctx, A, M, K, TC_BM, tc_box_k(256));
+  if (!rc) rc = tc_alloc(&ctx, B, N, K, 256, tc_box_k(256));
+  if (!rc) rc = tc_set_attrs();
+  if (!rc) {
+    split16(&ctx, 0, dA, 1.0f, A.hi, A.lo, (size_t)M * K);
+    split16(&ctx, 0, dB, 64.0f, B.hi, B.lo, (size_t)N * K);
+    gemm_tc_gru(&ctx, 0, A, B, M, dbias, h_in, mask, h_out, group, pitch, off, out_hi, out_lo, ldh);
+    cudaError_t err = cudaDeviceSynchronize();
+    if (err != cudaSuccess) rc = cn_set_error("cn_internal_gemm_tc_gru: %s", cudaGetErrorString(err));
+    else if (ctx.launch_error) rc = 1;
+  }
+  cn_launch_free(&ctx);
+  return rc;
+}
 
 #ifdef CN_GEMM_TRACE
 // Traced builds only (tools/gemm_tile_trace.py): every following gemm_tc launch writes per-tile records
