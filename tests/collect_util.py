@@ -1,23 +1,14 @@
 """Shared pieces of the data-collection tests (CrowdSimVarNumCollect-v0): the golden cases recorded by
 tools/make_golden_collect.py, their engine configuration, a replay through any engine with reset() / step(actions) /
-get(name), and the host build of the collect step (tests/cpu_harness/collect_harness.cpp)."""
+get(name)."""
 import ast
-import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from crowdnav_prediction_attngraph_b200 import _capi
-from tests import harness_util
 from tests.golden_util import GOLD
-from tests.harness_util import HarnessEnv
 
 COLLECT_CASES = ["collect_h20_train", "collect_h8_sf_humans", "collect_h10_sf_robot"]
-COLLECT_SO = os.path.join(harness_util.HERE, "_build_collect_harness.so")
-COLLECT_SRC = os.path.join(harness_util.HERE, "cpu_harness", "collect_harness.cpp")
-STATE_DTYPES = dict(harness_util.STATE_DTYPES, rwx="f8", rwy="f8", rsim_exists="u1", rsim_nd="f4", rsim_rother="f4",
-                    pred_id="i4", max_id="i4", rgoal_due="u1", rgoal_med="f8")
 
 
 def load_collect_case(name):
@@ -71,50 +62,3 @@ def replay_collect(g, reset_fn, step_fn, get_fn, pos_tol=1e-9):
         if msg:
             bad.append("t=%d: %s" % (t, ",".join(msg)))
     return bad
-
-
-def _build():
-    core = harness_util.CORE
-    deps = [COLLECT_SRC, harness_util.SRC, os.path.join(harness_util.HERE, "cpu_harness", "robot_harness.cpp")] + \
-        [os.path.join(core, f) for f in os.listdir(core) if f.endswith(".cuh")]
-    if os.path.exists(COLLECT_SO) and all(os.path.getmtime(COLLECT_SO) >= os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-o", COLLECT_SO,
-                           COLLECT_SRC])
-
-
-class CollectHarnessEnv(HarnessEnv):
-    """N collect environments stepped by the host build of the kernel logic; reset() / step() return pred_info."""
-
-    def __init__(self, **cfg_over):
-        super().__init__(**cfg_over)
-        self.lib.harness_destroy(self.h)
-        self.h = None
-        _build()
-        old, lib = self.lib, C.CDLL(COLLECT_SO)
-        for name in ("harness_destroy", "harness_state_bytes", "harness_state_copy"):
-            f, o = getattr(lib, name), getattr(old, name)
-            f.argtypes, f.restype = o.argtypes, o.restype
-        lib.collect_harness_create.restype = C.c_void_p
-        lib.collect_harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
-        lib.collect_harness_reset.argtypes = [C.c_void_p, C.c_void_p]
-        lib.collect_harness_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(_capi.CnStepPtrs)]
-        self.lib = lib
-        self.h = lib.collect_harness_create(C.byref(self.cfg))
-        self.pred_info = np.zeros((self.N, self.H, 4), np.float32)
-
-    def reset(self):
-        self.lib.collect_harness_reset(self.h, self.pred_info.ctypes.data)
-        return self.pred_info.copy()
-
-    def step(self, actions):
-        a = np.ascontiguousarray(actions, dtype=np.float32)
-        self.lib.collect_harness_step(self.h, a.ctypes.data, self.pred_info.ctypes.data, C.byref(self.outp))
-        return self.pred_info.copy(), {k: v.copy() for k, v in self.out.items()}
-
-    def get(self, name):
-        nbytes = self.lib.harness_state_bytes(self.h, name.encode())
-        assert nbytes, name
-        arr = np.zeros(nbytes // np.dtype(STATE_DTYPES[name]).itemsize, STATE_DTYPES[name])
-        assert self.lib.harness_state_copy(self.h, name.encode(), arr.ctypes.data, nbytes, 0) == 0
-        return arr

@@ -1,4 +1,4 @@
-"""Test helper: drives the HOST build of the step-kernel logic (tests/cpu_harness) through the
+"""Test helper: drives the HOST build of the step-kernel logic (tests/cpu_harness/env_harness.cpp) through the
 same struct layouts as the C ABI.  Test infrastructure only."""
 import ctypes as C
 import os
@@ -19,7 +19,10 @@ STATE_DTYPES = dict(
     hpx="f8", hpy="f8", hgx="f8", hgy="f8", hrad="f8", hvpref="f8", hvx="f4", hvy="f4",
     bpx="f8", bpy="f8", bvx="f8", bvy="f8", brad="f8", vis="u1", sim_exists="u1",
     sim_nd="f4", sim_rself="f4", sim_vmax="f4", sim_rother="f4", mt="u4", mt_pos="i4",
-    last_hvx="f4", last_hvy="f4", orca_nlines="i4", orca_fail="i4", evt="u1", spawn_overflow="u1", hn="i4", prep_hn="i4")
+    last_hvx="f4", last_hvy="f4", orca_nlines="i4", orca_fail="i4", evt="u1", spawn_overflow="u1", hn="i4", prep_hn="i4",
+    sim_n="u1", hwx="f8", hwy="f8",
+    rwx="f8", rwy="f8", rsim_exists="u1", rsim_nd="f4", rsim_rother="f4",
+    pred_id="i4", max_id="i4", rgoal_due="u1", rgoal_med="f8")
 
 
 def build():
@@ -30,34 +33,42 @@ def build():
 
 
 class HarnessEnv(object):
-    """N environments stepped by the host build of the kernel logic."""
+    """N environments stepped by the host build of the kernel logic, configured like cn_env_create (robot policy,
+    robot.visible, social-force humans, phase 'test', 'truth' observations).  collect=True: the collect environment
+    (cn_env_create_collect), whose reset() / step() return pred_info instead of the observation dict."""
 
-    def __init__(self, **cfg_over):
+    def __init__(self, collect=False, **cfg_over):
         build()
         self.lib = C.CDLL(SO)
         self.lib.harness_create.restype = C.c_void_p
-        self.lib.harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
+        self.lib.harness_create.argtypes = [C.POINTER(_capi.CnConfig), C.c_int]
         self.lib.harness_destroy.argtypes = [C.c_void_p]
-        self.lib.harness_reset.argtypes = [C.c_void_p, C.POINTER(_capi.CnObsPtrs)]
+        self.lib.harness_reset.argtypes = [C.c_void_p, C.POINTER(_capi.CnObsPtrs), C.c_void_p]
         self.lib.harness_step.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(_capi.CnObsPtrs),
-                                          C.POINTER(_capi.CnStepPtrs)]
+                                          C.POINTER(_capi.CnStepPtrs), C.c_void_p]
         self.lib.harness_state_bytes.restype = C.c_size_t
         self.lib.harness_state_bytes.argtypes = [C.c_void_p, C.c_char_p]
         self.lib.harness_state_copy.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t, C.c_int]
         self.cfgd = _capi.default_config_dict(**cfg_over)
         self.cfg = _capi.config_from_dict(self.cfgd)
-        self.h = self.lib.harness_create(C.byref(self.cfg))
+        self.collect = collect
+        self.h = self.lib.harness_create(C.byref(self.cfg), int(collect))
         N, H = self.cfgd["num_envs"], self.cfgd["human_num"] + self.cfgd["human_num_range"]
         W = 2 * (self.cfgd["predict_steps"] + 1) if self.cfgd["const_vel"] else 2
         self.N, self.H, self.W = N, H, W
-        self.ob = dict(robot_node=np.zeros((N, 1, 7), np.float32), temporal_edges=np.zeros((N, 1, 2), np.float32),
-                       spatial_edges=np.zeros((N, H, W), np.float32), detected_human_num=np.zeros((N, 1), np.float32))
-        if not self.cfgd["const_vel"]:
-            self.ob["visible_masks"] = np.zeros((N, H), np.uint8)
+        if collect:
+            self.pred_info = np.zeros((N, H, 4), np.float32)
+            self.obp, self.pip = None, self.pred_info.ctypes.data
+        else:
+            self.ob = dict(robot_node=np.zeros((N, 1, 7), np.float32), temporal_edges=np.zeros((N, 1, 2), np.float32),
+                           spatial_edges=np.zeros((N, H, W), np.float32), detected_human_num=np.zeros((N, 1), np.float32))
+            if not self.cfgd["const_vel"]:
+                self.ob["visible_masks"] = np.zeros((N, H), np.uint8)
+            self.obp = C.pointer(_capi.CnObsPtrs(*[self.ob[k].ctypes.data if k in self.ob else None
+                                                   for k, _ in _capi.CnObsPtrs._fields_]))
+            self.pip = None
         self.out = dict(reward=np.zeros(N, np.float32), done=np.zeros(N, np.uint8), info=np.zeros(N, np.int32),
                         info_aux=np.zeros(N, np.float32), ep_ret=np.zeros(N, np.float64), ep_len=np.zeros(N, np.int32))
-        self.obp = _capi.CnObsPtrs(*[self.ob[k].ctypes.data if k in self.ob else None
-                                     for k, _ in _capi.CnObsPtrs._fields_])
         self.outp = _capi.CnStepPtrs(*[self.out[k].ctypes.data if k in self.out else None
                                        for k, _ in _capi.CnStepPtrs._fields_])
 
@@ -67,18 +78,20 @@ class HarnessEnv(object):
             self.h = None
 
     def _obs(self):
+        if self.collect:
+            return self.pred_info.copy()
         o = {k: v.copy() for k, v in self.ob.items()}
         if "visible_masks" in o:
             o["visible_masks"] = o["visible_masks"].astype(bool)
         return o
 
     def reset(self):
-        self.lib.harness_reset(self.h, C.byref(self.obp))
+        self.lib.harness_reset(self.h, self.obp, self.pip)
         return self._obs()
 
     def step(self, actions):
         a = np.ascontiguousarray(actions, dtype=np.float32)
-        self.lib.harness_step(self.h, a.ctypes.data, C.byref(self.obp), C.byref(self.outp))
+        self.lib.harness_step(self.h, a.ctypes.data, self.obp, C.byref(self.outp), self.pip)
         return self._obs(), {k: v.copy() for k, v in self.out.items()}
 
     def get(self, name):

@@ -1,54 +1,8 @@
 """Shared pieces of the robot-policy tests (robot.policy 'orca' / 'social_force'): the golden cases, a replay of
-them through any engine with reset() / step(actions) / get(name) that also checks the robot's velocity, and the host
-build of the step kernel's logic with the robot's policy (tests/cpu_harness/robot_harness.cpp)."""
-import ctypes as C
-import os
-import subprocess
-
+them through any engine with reset() / step(actions) / get(name) that also checks the robot's velocity."""
 import numpy as np
 
-from crowdnav_prediction_attngraph_b200 import _capi
-from tests import harness_util
 from tests.golden_util import load_env_case, replay
-from tests.harness_util import HarnessEnv
-
-ROBOT_SO = os.path.join(harness_util.HERE, "_build_robot_harness.so")
-ROBOT_SRC = os.path.join(harness_util.HERE, "cpu_harness", "robot_harness.cpp")
-STATE_DTYPES = dict(harness_util.STATE_DTYPES, rwx="f8", rwy="f8", rsim_exists="u1", rsim_nd="f4", rsim_rother="f4")
-
-
-def _build_robot_harness():
-    core = harness_util.CORE
-    deps = [ROBOT_SRC, harness_util.SRC] + [os.path.join(core, f) for f in os.listdir(core) if f.endswith(".cuh")]
-    if os.path.exists(ROBOT_SO) and all(os.path.getmtime(ROBOT_SO) >= os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-o", ROBOT_SO, ROBOT_SRC])
-
-
-class RobotHarnessEnv(HarnessEnv):
-    """HarnessEnv whose environments run cn_config.robot_policy (robot_harness_create): same buffers and entry points,
-    plus the robot's state fields."""
-
-    def __init__(self, **cfg_over):
-        super().__init__(**cfg_over)
-        self.lib.harness_destroy(self.h)
-        self.h = None
-        _build_robot_harness()
-        old, lib = self.lib, C.CDLL(ROBOT_SO)
-        for name in ("harness_destroy", "harness_reset", "harness_step", "harness_state_bytes", "harness_state_copy"):
-            f, o = getattr(lib, name), getattr(old, name)
-            f.argtypes, f.restype = o.argtypes, o.restype
-        lib.robot_harness_create.restype = C.c_void_p
-        lib.robot_harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
-        self.lib = lib
-        self.h = lib.robot_harness_create(C.byref(self.cfg))
-
-    def get(self, name):
-        nbytes = self.lib.harness_state_bytes(self.h, name.encode())
-        assert nbytes, name
-        arr = np.zeros(nbytes // np.dtype(STATE_DTYPES[name]).itemsize, STATE_DTYPES[name])
-        assert self.lib.harness_state_copy(self.h, name.encode(), arr.ctypes.data, nbytes, 0) == 0
-        return arr
 
 ROBOT_CASES = ["env_varnum_h20_test_orca_robot", "env_varnum_h10_orca_robot_rand",
                "env_varnum_h20_test_sf_robot", "env_varnum_h10_sf_robot_rand"]

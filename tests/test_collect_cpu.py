@@ -6,14 +6,15 @@ import os
 import numpy as np
 import pytest
 
-from tests.collect_util import COLLECT_CASES, CollectHarnessEnv, load_collect_case, replay_collect
+from tests.collect_util import COLLECT_CASES, load_collect_case, replay_collect
 from tests.golden_util import GOLD
+from tests.harness_util import HarnessEnv
 
 
 @pytest.mark.parametrize("name", COLLECT_CASES)
 def test_collect_kernel_logic_host_build_matches_reference_golden(name):
     g, case, over = load_collect_case(name)
-    env = CollectHarnessEnv(**over)
+    env = HarnessEnv(collect=True, **over)
     bad = replay_collect(g, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 

@@ -1,58 +1,16 @@
 """robot.visible = True (the humans' ORCA / social-force solves see the robot) in the host build of the step kernel's
-logic (tests/cpu_harness/vis_harness.cpp), replayed against goldens recorded from the unmodified reference (tools/make_golden.py):
+logic (tests/cpu_harness/env_harness.cpp), replayed against goldens recorded from the unmodified reference (tools/make_golden.py):
 bit-exact done / info / ORCA velocities / line counts / failure index / sim_exists, fp64 state within 1e-9.  Also the
 config mapping of robot.visible."""
 import copy
-import ctypes as C
-import os
-import subprocess
 import types
 
 import numpy as np
 import pytest
 
-from crowdnav_prediction_attngraph_b200 import _capi
-from tests import harness_util
 from tests.golden_util import load_env_case, replay
 from tests.harness_util import HarnessEnv
-from tests.robot_policy_util import ROBOT_POLICY, ROBOT_SRC, STATE_DTYPES, replay_robot
-
-VIS_SO = os.path.join(harness_util.HERE, "_build_vis_harness.so")
-VIS_SRC = os.path.join(harness_util.HERE, "cpu_harness", "vis_harness.cpp")
-
-
-def _build_vis_harness():
-    core = harness_util.CORE
-    deps = [VIS_SRC, ROBOT_SRC, harness_util.SRC] + [os.path.join(core, f) for f in os.listdir(core) if f.endswith(".cuh")]
-    if os.path.exists(VIS_SO) and all(os.path.getmtime(VIS_SO) >= os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-o", VIS_SO, VIS_SRC])
-
-
-class VisHarnessEnv(HarnessEnv):
-    """HarnessEnv whose environments run cn_config.robot_visible (and robot_policy: vis_harness_create): same buffers
-    and entry points, plus the robot's state fields."""
-
-    def __init__(self, **cfg_over):
-        super().__init__(**cfg_over)
-        self.lib.harness_destroy(self.h)
-        self.h = None
-        _build_vis_harness()
-        old, lib = self.lib, C.CDLL(VIS_SO)
-        for name in ("harness_destroy", "harness_reset", "harness_step", "harness_state_bytes", "harness_state_copy"):
-            f, o = getattr(lib, name), getattr(old, name)
-            f.argtypes, f.restype = o.argtypes, o.restype
-        lib.vis_harness_create.restype = C.c_void_p
-        lib.vis_harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
-        self.lib = lib
-        self.h = lib.vis_harness_create(C.byref(self.cfg))
-
-    def get(self, name):
-        nbytes = self.lib.harness_state_bytes(self.h, name.encode())
-        assert nbytes, name
-        arr = np.zeros(nbytes // np.dtype(STATE_DTYPES[name]).itemsize, STATE_DTYPES[name])
-        assert self.lib.harness_state_copy(self.h, name.encode(), arr.ctypes.data, nbytes, 0) == 0
-        return arr
+from tests.robot_policy_util import ROBOT_POLICY, replay_robot
 
 # train (config-1 shape; randomised with goal changes, episode ends crossed), test phase (simulators rebuilt on every
 # agent-count change), humans joining / leaving (the robot's index follows the live count), social-force humans,
@@ -76,7 +34,7 @@ def load_vis_case(name):
 @pytest.mark.parametrize("name", VIS_CASES)
 def test_kernel_logic_host_build_robot_visible_matches_reference_golden(name):
     g, case, over = load_vis_case(name)
-    env = VisHarnessEnv(**over)
+    env = HarnessEnv(**over)
     bad = replay(g, case, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 
@@ -84,7 +42,7 @@ def test_kernel_logic_host_build_robot_visible_matches_reference_golden(name):
 @pytest.mark.parametrize("name", VIS_ROBOT_CASES)
 def test_kernel_logic_host_build_robot_visible_orca_robot_matches_reference_golden(name):
     g, case, over = load_vis_case(name)
-    env = VisHarnessEnv(**over)
+    env = HarnessEnv(**over)
     bad = replay_robot(g, case, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 

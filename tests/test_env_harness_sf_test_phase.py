@@ -1,25 +1,19 @@
 """Social-force humans (humans.policy = 'social_force') in phase 'test' on the CPU: the host build of the step kernel's
-logic with the social-force look-ahead (tests/cpu_harness/sf_test_harness.cpp, on top of the robot / robot-visible
-builds) and the oracle (oracle/crowd_env.py) against goldens recorded from the unmodified reference (tools/make_golden.py).  In phase 'test'
-the step runs the ground-truth look-ahead calc_human_future_traj('truth') with SOCIAL_FORCE.predict on the humans only,
-fp64, and its kept rows feed the 'future' danger zone and, on CrowdSimPred-v0, the future-collision penalty.  Also the
-config mapping: one environment gives phase 'test' with social-force humans."""
-import ctypes as C
-import os
-import subprocess
+logic with the social-force look-ahead (tests/cpu_harness/env_harness.cpp) and the oracle (oracle/crowd_env.py)
+against goldens recorded from the unmodified reference (tools/make_golden.py).  In phase 'test' the step runs the
+ground-truth look-ahead calc_human_future_traj('truth') with SOCIAL_FORCE.predict on the humans only, fp64, and its
+kept rows feed the 'future' danger zone and, on CrowdSimPred-v0, the future-collision penalty.  Also the config mapping:
+one environment gives phase 'test' with social-force humans."""
 import types
 
 import numpy as np
 import pytest
 
-from crowdnav_prediction_attngraph_b200 import _capi
 from oracle.crowd_env import CrowdEnvOracle, EnvConfig
-from tests import harness_util
 from tests.golden_util import load_env_case, replay
 from tests.harness_util import HarnessEnv
 from tests.robot_oracle import RobotPolicyOracle
-from tests.robot_policy_util import ROBOT_POLICY, ROBOT_SRC, STATE_DTYPES, replay_robot
-from tests.test_env_harness_robot_visible import VIS_SRC
+from tests.robot_policy_util import ROBOT_POLICY, replay_robot
 
 # CrowdSimVarNum-v0 (8 randomised humans, goal changes), CrowdSimPred-v0 (10 randomised humans: future penalty and
 # 'future' danger zone together), the first with robot.visible (the real solve sees the robot, the look-ahead does
@@ -28,51 +22,6 @@ SF_TEST_CASES = ["env_varnum_h8_sf_test_rand", "env_pred_h10_sf_test_rand", "env
                  "env_varnum_h6_range2_sf_test"]
 # the ORCA and the social-force robot among 20 social-force humans
 SF_TEST_ROBOT_CASES = ["env_varnum_h20_test_sf_humans_orca_robot", "env_varnum_h20_test_sf_humans_sf_robot"]
-
-SF_SO = os.path.join(harness_util.HERE, "_build_sf_test_harness.so")
-SF_SRC = os.path.join(harness_util.HERE, "cpu_harness", "sf_test_harness.cpp")
-
-
-def _build_sf_harness():
-    core = harness_util.CORE
-    deps = [SF_SRC, VIS_SRC, ROBOT_SRC, harness_util.SRC] + \
-        [os.path.join(core, f) for f in os.listdir(core) if f.endswith(".cuh")]
-    if os.path.exists(SF_SO) and all(os.path.getmtime(SF_SO) >= os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-o", SF_SO, SF_SRC])
-
-
-class SfTestHarnessEnv(HarnessEnv):
-    """HarnessEnv of social-force humans in phase 'test' (robot policy and robot.visible as vis_harness_create takes
-    them): the same buffers and entry points, with sf_harness_step (the social-force look-ahead) as the step."""
-
-    def __init__(self, **cfg_over):
-        super().__init__(**cfg_over)
-        self.lib.harness_destroy(self.h)
-        self.h = None
-        _build_sf_harness()
-        old, lib = self.lib, C.CDLL(SF_SO)
-        for name in ("harness_destroy", "harness_reset", "harness_state_bytes", "harness_state_copy"):
-            f, o = getattr(lib, name), getattr(old, name)
-            f.argtypes, f.restype = o.argtypes, o.restype
-        lib.vis_harness_create.restype = C.c_void_p
-        lib.vis_harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
-        lib.sf_harness_step.restype = C.c_int
-        lib.sf_harness_step.argtypes = old.harness_step.argtypes
-        self.lib = lib
-        self.h = lib.vis_harness_create(C.byref(self.cfg))
-
-    def step(self, actions):
-        a = np.ascontiguousarray(actions, dtype=np.float32)
-        assert self.lib.sf_harness_step(self.h, a.ctypes.data, C.byref(self.obp), C.byref(self.outp)) == 0
-        return self._obs(), {k: v.copy() for k, v in self.out.items()}
-
-    def get(self, name):
-        nbytes = self.lib.harness_state_bytes(self.h, name.encode())
-        assert nbytes, name
-        arr = np.zeros(nbytes // np.dtype(STATE_DTYPES[name]).itemsize, STATE_DTYPES[name])
-        assert self.lib.harness_state_copy(self.h, name.encode(), arr.ctypes.data, nbytes, 0) == 0
-        return arr
 
 
 def load_sf_test_case(name):
@@ -94,7 +43,7 @@ def test_fixture_is_sf_test_phase_with_episode_ends_and_danger(name):
 @pytest.mark.parametrize("name", SF_TEST_CASES)
 def test_kernel_logic_host_build_sf_test_phase_matches_reference_golden(name):
     g, case, over = load_sf_test_case(name)
-    env = SfTestHarnessEnv(**over)
+    env = HarnessEnv(**over)
     bad = replay(g, case, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 
@@ -102,7 +51,7 @@ def test_kernel_logic_host_build_sf_test_phase_matches_reference_golden(name):
 @pytest.mark.parametrize("name", SF_TEST_ROBOT_CASES)
 def test_kernel_logic_host_build_sf_test_phase_robot_matches_reference_golden(name):
     g, case, over = load_sf_test_case(name)
-    env = SfTestHarnessEnv(**over)
+    env = HarnessEnv(**over)
     bad = replay_robot(g, case, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 

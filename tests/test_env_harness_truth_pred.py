@@ -1,5 +1,5 @@
 """CrowdSimPred-v0 with sim.predict_method = 'truth' on the CPU: the host build of the step kernel's logic with the
-observation look-ahead (tests/cpu_harness/truth_harness.cpp) and the oracle (tests/truth_oracle.py) against goldens
+observation look-ahead (tests/cpu_harness/env_harness.cpp) and the oracle (tests/truth_oracle.py) against goldens
 recorded from the unmodified reference (tools/make_golden.py).  Every observation, the first of an episode included,
 runs calc_human_future_traj('truth'): buffer_len nested solves of the live humans from their true state, the kept rows
 of the humans the robot sees as observation columns and as the trajectory the next step's reward penalises.  The
@@ -7,7 +7,6 @@ look-ahead is often the call that creates a human's rvo2 simulator (after a rese
 every step), freezing every human's true radius.  Also the config mapping and the configurations still refused."""
 import ctypes as C
 import os
-import subprocess
 import types
 
 import numpy as np
@@ -15,12 +14,8 @@ import pytest
 
 from crowdnav_prediction_attngraph_b200 import _capi
 from oracle.crowd_env import EnvConfig
-from tests import harness_util
 from tests.golden_util import GOLD, load_env_case, replay
 from tests.harness_util import HarnessEnv
-from tests.robot_policy_util import ROBOT_SRC
-from tests.test_env_harness_robot_visible import VIS_SRC
-from tests.test_env_harness_sf_test_phase import SF_SRC
 from tests.truth_oracle import TruthPredOracle
 
 # phase 'train' (the next step's reward reads the observed trajectory) and 'test' (two look-aheads per step), ORCA and
@@ -29,59 +24,6 @@ from tests.truth_oracle import TruthPredOracle
 TRUTH_CASES = ["env_pred_h20_truth", "env_pred_h10_truth_rand", "env_pred_h10_truth_test_rand", "env_pred_h6_range3_truth",
                "env_pred_h10_truth_vis_rand", "env_pred_h10_truth_test_vis_rand", "env_pred_h8_sf_truth_rand",
                "env_pred_h8_sf_truth_test_rand"]
-
-TRUTH_SO = os.path.join(harness_util.HERE, "_build_truth_harness.so")
-TRUTH_SRC = os.path.join(harness_util.HERE, "cpu_harness", "truth_harness.cpp")
-STATE_DTYPES = dict(harness_util.STATE_DTYPES, hwx="f8", hwy="f8", sim_n="u1")
-
-
-def _build_truth_harness():
-    core = harness_util.CORE
-    deps = [TRUTH_SRC, SF_SRC, VIS_SRC, ROBOT_SRC, harness_util.SRC] + \
-        [os.path.join(core, f) for f in os.listdir(core) if f.endswith(".cuh")]
-    if os.path.exists(TRUTH_SO) and all(os.path.getmtime(TRUTH_SO) >= os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-shared", "-o", TRUTH_SO, TRUTH_SRC])
-
-
-class TruthHarnessEnv(HarnessEnv):
-    """HarnessEnv of CrowdSimPred-v0 / 'truth' (robot.visible as vis_harness_create takes it): the same buffers, with
-    truth_harness_reset / truth_harness_step (the observation look-ahead) as reset and step."""
-
-    def __init__(self, **cfg_over):
-        cfg_over.setdefault("const_vel", 2)
-        super().__init__(**cfg_over)
-        self.lib.harness_destroy(self.h)
-        self.h = None
-        _build_truth_harness()
-        old, lib = self.lib, C.CDLL(TRUTH_SO)
-        for name in ("harness_destroy", "harness_state_bytes", "harness_state_copy"):
-            f, o = getattr(lib, name), getattr(old, name)
-            f.argtypes, f.restype = o.argtypes, o.restype
-        lib.truth_harness_create.restype = C.c_void_p
-        lib.truth_harness_create.argtypes = [C.POINTER(_capi.CnConfig)]
-        lib.truth_harness_reset.restype = C.c_int
-        lib.truth_harness_reset.argtypes = old.harness_reset.argtypes
-        lib.truth_harness_step.restype = C.c_int
-        lib.truth_harness_step.argtypes = old.harness_step.argtypes
-        self.lib = lib
-        self.h = lib.truth_harness_create(C.byref(self.cfg))
-
-    def reset(self):
-        assert self.lib.truth_harness_reset(self.h, C.byref(self.obp)) == 0
-        return self._obs()
-
-    def step(self, actions):
-        a = np.ascontiguousarray(actions, dtype=np.float32)
-        assert self.lib.truth_harness_step(self.h, a.ctypes.data, C.byref(self.obp), C.byref(self.outp)) == 0
-        return self._obs(), {k: v.copy() for k, v in self.out.items()}
-
-    def get(self, name):
-        nbytes = self.lib.harness_state_bytes(self.h, name.encode())
-        assert nbytes, name
-        arr = np.zeros(nbytes // np.dtype(STATE_DTYPES[name]).itemsize, STATE_DTYPES[name])
-        assert self.lib.harness_state_copy(self.h, name.encode(), arr.ctypes.data, nbytes, 0) == 0
-        return arr
 
 
 def load_truth_case(name):
@@ -157,7 +99,7 @@ def test_kernel_logic_host_build_truth_matches_reference_golden(name):
     look-ahead's) and simulator existence bit for bit; observations, rewards and state at the replay's tolerances; the
     future-collision penalty the next reward reads, against the trajectory the reference stored."""
     g, case, over = load_truth_case(name)
-    env = TruthHarnessEnv(**over)
+    env = HarnessEnv(**over)
     trajs = recorded_trajectories(g)
     pen_bad, t_box = [], [0]
 

@@ -17,8 +17,9 @@ import pytest
 import torch
 
 from tests.golden_util import replay
+from tests.harness_util import HarnessEnv
 from tests.robot_policy_util import replay_robot
-from tests.test_env_harness_robot_visible import VIS_CASES, VIS_ROBOT_CASES, VisHarnessEnv, load_vis_case
+from tests.test_env_harness_robot_visible import VIS_CASES, VIS_ROBOT_CASES, load_vis_case
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -92,7 +93,7 @@ def _lockstep_vs_harness(N, T, offsets, tol=1e-9, **over):
     """CUDA engine of N environments vs the host build run as single-environment shards at the given rank offsets;
     environments whose spawn search overflowed (the reference would spin there) are excluded."""
     env = _engine(num_envs=N, nenv_total=N, **over)
-    hs = [VisHarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
+    hs = [HarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
     idx = np.array(offsets)
     H = env.human_num
     env.reset()

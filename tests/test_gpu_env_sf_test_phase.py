@@ -17,8 +17,9 @@ import pytest
 import torch
 
 from tests.golden_util import replay
+from tests.harness_util import HarnessEnv
 from tests.robot_policy_util import replay_robot
-from tests.test_env_harness_sf_test_phase import SF_TEST_CASES, SF_TEST_ROBOT_CASES, SfTestHarnessEnv, load_sf_test_case
+from tests.test_env_harness_sf_test_phase import SF_TEST_CASES, SF_TEST_ROBOT_CASES, load_sf_test_case
 from tests.test_gpu_env_robot_visible import _np_obs, _policy, _step_fn
 
 pytestmark = pytest.mark.gpu
@@ -62,7 +63,7 @@ def _lockstep_vs_harness(N, T, offsets, tol=1e-9, **over):
     Returns (compared environment-steps, velocities that were not bit for bit equal)."""
     from crowdnav_prediction_attngraph_b200.vec_env import CudaCrowdVecEnv
     env = CudaCrowdVecEnv(device="cuda:0", num_envs=N, nenv_total=N, **over)
-    hs = [SfTestHarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
+    hs = [HarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
     H = env.human_num
     env.reset()
     for h in hs:

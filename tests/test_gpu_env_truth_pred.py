@@ -5,7 +5,7 @@ cn_env_step_kernel): every observation runs the ground-truth look-ahead and obse
     stream, and with every rejection-sampling search sent to the CTA-scope event kernel (CN_DEFER_TRIES=1), including
     the future-collision penalty the next step's reward reads against the trajectory the reference stored;
   * over 220 steps through episode ends, environments picked by rank offset match the host build
-    (tests/cpu_harness/truth_harness.cpp) step for step: 4096 x 20 humans, 50 and 100 humans (the three MAXH
+    (tests/cpu_harness/env_harness.cpp) step for step: 4096 x 20 humans, 50 and 100 humans (the three MAXH
     instantiations), 128 slots with the robot visible, humans joining and leaving, phase 'test', social-force humans;
   * the batched evaluation equals the sequential protocol;
   * a device-resident rollout of the attention-graph policy and one PPO.update give finite results;
@@ -17,8 +17,9 @@ import pytest
 import torch
 
 from tests.golden_util import replay
-from tests.test_env_harness_truth_pred import (TRUTH_CASES, FinishedEpisodeDiagnosticsMasked, TruthHarnessEnv,
-                                               future_penalty, load_truth_case, recorded_trajectories)
+from tests.harness_util import HarnessEnv
+from tests.test_env_harness_truth_pred import (TRUTH_CASES, FinishedEpisodeDiagnosticsMasked, future_penalty,
+                                               load_truth_case, recorded_trajectories)
 from tests.test_gpu_env_robot_visible import _np_obs, _step_fn
 
 pytestmark = pytest.mark.gpu
@@ -82,7 +83,7 @@ def _lockstep_vs_harness(N, T, offsets, tol=1e-9, **over):
     glibc's differ in the last bit now and then, see tests/test_gpu_env_sf_test_phase.py).  Returns the compared
     environment-steps."""
     env = _engine(num_envs=N, nenv_total=N, **over)
-    hs = [TruthHarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
+    hs = [HarnessEnv(num_envs=1, nenv_total=N, rank_offset=r, **over) for r in offsets]
     H = env.human_num
     sf = over.get("human_policy", 0) == 1
     ob = _np_obs(env.reset())

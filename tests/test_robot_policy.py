@@ -8,8 +8,9 @@ import numpy as np
 import pytest
 
 from oracle.crowd_env import EnvConfig
+from tests.harness_util import HarnessEnv
 from tests.robot_oracle import RobotPolicyOracle
-from tests.robot_policy_util import ROBOT_CASES, RobotHarnessEnv, load_robot_case, replay_robot
+from tests.robot_policy_util import ROBOT_CASES, load_robot_case, replay_robot
 from tests.test_oracle_golden import check_state
 
 
@@ -47,7 +48,7 @@ def test_oracle_robot_policy_matches_reference_golden(name):
 @pytest.mark.parametrize("name", ROBOT_CASES)
 def test_kernel_logic_host_build_robot_policy_matches_reference_golden(name):
     g, case, over = load_robot_case(name)
-    env = RobotHarnessEnv(**over)
+    env = HarnessEnv(**over)
     bad = replay_robot(g, case, env.reset, env.step, env.get)
     assert not bad, bad[:5]
 
